@@ -34,8 +34,6 @@
 #include "../../include/b200mj_convex.h"
 
 #define FULL 0xffffffffu
-#define B200MJ_INTERNAL_ACC_SYNC (1 << 16)     // host -> acceleration kernels only (not part of the ABI flags)
-#define B200MJ_INTERNAL_ACC_SYNC_COARSE (1 << 17)   // barriers at the stage boundaries only, Newton trips run free
 #define FOR_LANES(i, n) _Pragma("unroll 1") for (int i = lane; i < (n); i += 32)
 
 // ------------------------------------------------------------------------------------------------
@@ -51,9 +49,6 @@ struct DevModel {
   // actuator moments by dof (CSR, built by b200mj_model_create): joint and fixed-tendon transmissions have constant
   // moment arms, so qfrc_actuator[i] = sum over dof_act_id[dof_act_adr[i] .. dof_act_adr[i+1]) of coef * force
   const int* dof_act_adr; const int* dof_act_id; const double* dof_act_coef;
-  // dof tree (b200mj_model_create): ancestors of dof k, nearest first, at dof_anc_id[dof_anc_adr[k] .. dof_anc_adr[k+1]);
-  // dof_subsize[i] = dofs in the subtree of i, itself included (dofs are numbered depth-first: the subtree is i .. i+size-1)
-  const int* dof_anc_adr; const int* dof_anc_id; const int* dof_subsize;
   // per-environment geoms (b200mj_model_set_variable_geoms): geom_varid[g] = slot k of io.var_geom_pos / var_geom_size, or -1
   const int* geom_varid; int nvargeom;
   int ldv;          // padded row length of nv-wide matrices (odd => conflict-free column walks)
@@ -65,6 +60,7 @@ struct DevModel {
 
 // offsets (in doubles) into one environment's workspace
 struct Lay {
+  int total;                             // doubles per environment
   int qpos, qvel, act, ctrl, qaccws, actdot;
   int xpos, xquat, xmat, xipos, xanchor, xaxis, gxpos, gxmat, scom, slinvel;
   int cinert, crb, cdof, cdofdot, cvel, cacc, cfrc, cfrcext;
@@ -86,8 +82,6 @@ struct Lay {
   int dual, dV, dS, drows;
   int jalias;                            // dual form, small buckets: the workspace copy of J lives in H's storage (free once J M^-1 is there); J M^-1 is computed from the handover row
   int mglobal;                           // runtime-size acceleration kernels, nv >= 32: M stays in the handover row (no workspace copy)
-  int sparse;                            // ... and M, M + h B are factored as tree-sparse L'DL (ldl_factor) instead of dense Cholesky
-  int total;
 };
 
 // Per-environment row of the L2-resident handover buffer between the split position and acceleration kernels
@@ -99,31 +93,27 @@ struct Hand2 { int xpos, xquat, xmat, xipos, scom, cinert, cdof, cdofdot, cvel, 
 // Row-bucket compaction (split path): the position kernel appends every environment to the list of its row-count
 // bucket (count[b] = entries so far, list[b * cap ..]); the acceleration launch of a bucket then runs dense CTAs of
 // several warps over that list instead of one single-warp CTA per environment of which most exit at once.
-// Two classes per bucket by the Newton iteration count of the environment's previous physics step (a CTA lives as long
-// as its slowest warp: like with like): class 0 fills a bucket's list from the front (count[b]), class 1 from the back
-// (count[4 + b]).
-struct Compact { int* count; int* list; int cap; int nbucket; int rows_cap[4]; const int* prev_niter; int niter_split; int shadow_row; };
-#define SHADOW_ROWS 24   // private handover rows for the shadow warps of a launch's last CTA: [3 groups][8 warps]
+struct Compact { int* count; int* list; int cap; int nbucket; int rows_cap[4]; int shadow_row; };
+#define SHADOW_ROWS 16   // private handover rows for the shadow warps of a launch's last CTA: [2 groups][8 warps]
 
 struct b200mj_model {
   DevModel dm;
   Lay lay;
-  Lay lay_pos, lay_acc;       // compact workspaces of the split kernels (lay_acc: unused, kept for size queries)
+  Lay lay_pos;                // compact workspace of the split position kernels
   // acceleration kernel: row-count buckets (workspace sized for rows_cap[b] constraint rows), plain and
   // sensor-carrying (last physics step of a fused step) variants
   int nbucket; int rows_cap[4]; Lay lay_acc_b[4], lay_accs_b[4]; size_t smem_acc_b[4], smem_accs_b[4];
   Hand hand; Hand2 hand2;
   double* d_hand2;
   // environment groups x row buckets run on their own streams (independent work: hides each launch's tail)
-  cudaStream_t gmain[3], gaux[3][4]; cudaEvent_t ev_fork, ev_join[3], ev_pos[3], ev_acc[3][4]; int streams_ok;
+  cudaStream_t gmain[2], gaux[2][4]; cudaEvent_t ev_fork, ev_join[2], ev_pos[2], ev_acc[2][4]; int streams_ok;
   double* d_hand; int hand_batch;
   int convex_pairs;                // some candidate pair needs cvx_capsule_box / cvx_pair (else: primitive-only position kernels)
-  int* d_bcount; int* d_blist;     // compaction: counters [3 groups][BCOUNT_SLOTS][8], lists [3 groups][4 buckets][hand_batch]
-  int* d_niter;                    // Newton iterations of every environment's previous physics step [hand_batch]
+  int* d_bcount; int* d_blist;     // compaction: counters [2 groups][4 buckets], lists [2 groups][4 buckets][hand_batch]
   // the trailing mj_step1 of the last split-path step left a complete handover for this (io, batch): see B200MJ_STEP_REUSE_POS
   const double* reuse_qpos; int reuse_batch; int reuse_flags; int reuse_ok; int reuse_has_dump;
-  int epb_pos, epb_acc, pos_big;
-  size_t smem_pos, smem_acc;
+  int epb_pos, pos_big;
+  size_t smem_pos;
   int* d_idata;
   double* d_rdata;
   int* d_xi; double* d_xr;      // derived tables (dof_act_*)
@@ -132,6 +122,9 @@ struct b200mj_model {
   size_t smem_per_env;
   int tn_nv;                  // nv when a compile-time-size acceleration kernel exists for this model, else 0
   int nkey;
+  struct {                    // environment overrides for tests (read_test_hooks)
+    int tn, split, dual_min_nv, buckets[3], nbuckets, epb_pos, acc_warps, envs_per_block;
+  } hooks;
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -249,7 +242,8 @@ __device__ __forceinline__ int warp_excl_scan(int v, int lane, int* total) {
 }
 
 struct Ctx {
-  const DevModel& m; const Lay& L; double* ws; int lane; int disableflags; int sync_level;
+  const DevModel& m; const Lay& L; double* ws; int lane; int disableflags;
+  int newton_sync;      // every warp of the CTA takes the same number of Newton trips (multi-warp acceleration CTAs)
   // where the position/velocity stage deposits what the acceleration stage consumes: the workspace itself in the
   // fused kernel, this environment's row of the L2-resident handover buffer in the split position kernel
   double *pM, *pJ, *pD, *pAref, *pBias, *pPassive; int* pEq; double* stage;
@@ -257,7 +251,7 @@ struct Ctx {
   const double* Mc;     // acceleration stage: the joint-space inertia, read-only — the workspace copy, or (L.mglobal) the handover row in L2
   int env; const double* var_pos; const double* var_size;      // per-environment geoms (set_env)
   __device__ void set_env(int e, const b200mj_io& io) { env = e; var_pos = io.var_geom_pos; var_size = io.var_geom_size; }
-  __device__ Ctx(const DevModel& m_, const Lay& L_, double* ws_, int lane_, int df, int sl) : m(m_), L(L_), ws(ws_), lane(lane_), disableflags(df), sync_level(sl), env(0), var_pos(nullptr), var_size(nullptr) {
+  __device__ Ctx(const DevModel& m_, const Lay& L_, double* ws_, int lane_, int df, int ns) : m(m_), L(L_), ws(ws_), lane(lane_), disableflags(df), newton_sync(ns), env(0), var_pos(nullptr), var_size(nullptr) {
     pM = ws_ + L_.M; pJ = ws_ + L_.J; pD = ws_ + L_.efcD; pAref = ws_ + L_.aref; pBias = ws_ + L_.bias; pPassive = ws_ + L_.passive;
     pEq = reinterpret_cast<int*>(ws_ + L_.eqflag); stage = ws_ + L_.J; Mc = pM; Jg = pJ;
   }
@@ -611,96 +605,6 @@ __device__ __noinline__ void chol_solve_multi(const double* Lm, const double* di
 }
 
 // ------------------------------------------------------------------------------------------------
-// Tree-sparse L'DL of the joint-space inertia (what mj_factorM / mj_solveM do, O(sum depth^2) instead of O(nv^3)).
-// M[i][j] != 0 only when j is an ancestor of i in the dof tree, and eliminating dofs from the leaves up creates no
-// fill-in: M = L' D L with L unit lower triangular of the same pattern. For the CMU humanoid (62 dofs, depth <= 25)
-// that is 8 288 multiply-adds against 39 721 for the dense factorisation, and the substitutions walk 890 entries
-// instead of 1 953. The factor lives in the same packed lower triangle as the dense one; entries off the tree are never
-// touched. Stored: H[k][k] = D_k, H[k][i] = L[k][i] D_k (unscaled: the scaling by dinv[k] = 1 / D_k happens on use, which
-// saves a barrier per eliminated dof).
-//   ldl_factor: for k = nv-1 .. 0, the rank-1 update of k's ancestor block, lanes over the (ancestor, ancestor) pairs;
-//   ldl_solve:  L' pass (k descending, lanes over k's ancestors), D^-1, L pass (i ascending, lanes over i's subtree).
-// Used by the runtime-size acceleration kernels for nv >= 32 (c.L.sparse): M for qacc_smooth and the rows of J M^-1 of the
-// dual Newton form, M + h B for the Euler step. The Newton Hessian itself is dense (two touching limbs couple).
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tri_pair(int p, int& a, int& b) {      // p = b (b + 1) / 2 + a, a <= b
-  b = (int)((sqrtf(8.0f * (float)p + 1.0f) - 1.0f) * 0.5f);
-  while (((b + 1) * (b + 2)) >> 1 <= p) b++;
-  while ((b * (b + 1)) >> 1 > p) b--;
-  a = p - ((b * (b + 1)) >> 1);
-}
-
-__device__ __noinline__ void ldl_factor(const DevModel& m, double* H, double* dinv, int nv, int lane) {
-  _Pragma("unroll 1") for (int k = nv - 1; k >= 0; k--) {
-    const int a0 = m.dof_anc_adr[k], d = m.dof_anc_adr[k + 1] - a0;
-    const int* A = m.dof_anc_id + a0;
-    double* Hk = H + tri(k);
-    double Dk = Hk[k];
-    if (Dk < BMJ_MINVAL) Dk = BMJ_MINVAL;
-    const double inv = 1.0 / Dk;
-    if (lane == 0) dinv[k] = inv;
-    const int np = (d * (d + 1)) >> 1;
-    _Pragma("unroll 1") for (int p = lane; p < np; p += 32) {
-      int a, b; tri_pair(p, a, b);
-      const int i = A[a], j = A[b];      // j is i itself or one of its ancestors: j <= i < k
-      H[tri(i) + j] -= Hk[i] * inv * Hk[j];
-    }
-    __syncwarp();
-  }
-}
-
-// M x = b in place (x holds b on entry)
-__device__ __noinline__ void ldl_solve(const DevModel& m, const double* H, const double* dinv, double* x, int nv, int lane) {
-  __syncwarp();
-  _Pragma("unroll 1") for (int k = nv - 1; k > 0; k--) {        // x <- L^-T x
-    const int a0 = m.dof_anc_adr[k], d = m.dof_anc_adr[k + 1] - a0;
-    if (d == 0) continue;
-    const int* A = m.dof_anc_id + a0;
-    const double* Hk = H + tri(k);
-    const double xk = x[k] * dinv[k];
-    FOR_LANES(a, d) { const int i = A[a]; x[i] -= Hk[i] * xk; }
-    __syncwarp();
-  }
-  FOR_LANES(i, nv) x[i] *= dinv[i];
-  __syncwarp();
-  _Pragma("unroll 1") for (int i = 0; i < nv - 1; i++) {        // x <- L^-1 x: a finished x_i is pushed to its subtree
-    const int sz = m.dof_subsize[i];
-    if (sz <= 1) continue;
-    const double xi = x[i];
-    _Pragma("unroll 1") for (int k = i + 1 + lane; k < i + sz; k += 32) x[k] -= H[tri(k) + i] * dinv[k] * xi;
-    __syncwarp();
-  }
-}
-
-// M X = B for K right-hand sides (rows of stride ld), in place: the same three passes with lanes over (entry, right-hand side)
-__device__ __noinline__ void ldl_solve_multi(const DevModel& m, const double* H, const double* dinv, double* X, int ld, int K, int nv, int lane) {
-  int sh = 0;
-  while ((1 << sh) < K) sh++;                       // right-hand sides padded to a power of two: lane = (entry, rhs)
-  const int r = lane & ((1 << sh) - 1), e0 = lane >> sh, ne = 32 >> sh;
-  const bool on = r < K;
-  double* Xr = X + (on ? r : 0) * ld;
-  __syncwarp();
-  _Pragma("unroll 1") for (int k = nv - 1; k > 0; k--) {
-    const int a0 = m.dof_anc_adr[k], d = m.dof_anc_adr[k + 1] - a0;
-    if (d == 0) continue;
-    const int* A = m.dof_anc_id + a0;
-    const double* Hk = H + tri(k);
-    const double xk = on ? Xr[k] * dinv[k] : 0.0;
-    _Pragma("unroll 1") for (int a = e0; a < d; a += ne) if (on) { const int i = A[a]; Xr[i] -= Hk[i] * xk; }
-    __syncwarp();
-  }
-  _Pragma("unroll 1") for (int i = e0; i < nv; i += ne) if (on) Xr[i] *= dinv[i];
-  __syncwarp();
-  _Pragma("unroll 1") for (int i = 0; i < nv - 1; i++) {
-    const int sz = m.dof_subsize[i];
-    if (sz <= 1) continue;
-    const double xi = on ? Xr[i] : 0.0;
-    _Pragma("unroll 1") for (int k = i + 1 + e0; k < i + sz; k += ne) if (on) Xr[k] -= H[tri(k) + i] * dinv[k] * xi;
-    __syncwarp();
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
 // Compile-time-size dense algebra for the acceleration kernels (nv = N known at compile time, N <= 31).
 //
 // The runtime-size routines above walk the packed triangle in shared memory with rolled loops: 87 % of their
@@ -716,9 +620,6 @@ __device__ __noinline__ void ldl_solve_multi(const DevModel& m, const double* H,
 //     the diagonal zeroed: one shuffle + one DFMA per unknown, nothing else.
 // ------------------------------------------------------------------------------------------------
 #define TN_COLBUF_DOUBLES 64
-#ifndef TN_FACTOR_VARIANT
-#define TN_FACTOR_VARIANT 0
-#endif
 
 // 1/sqrt(x) for x in [mjMINVAL, huge): hardware seed + one cubic step, no special-case slow path (the library
 // rsqrt() carries a subroutine call for denormals / infinities, and a call inside the unrolled factorisation makes
@@ -767,7 +668,6 @@ __device__ __noinline__ void tn_factor(const double* Msrc, double* Lm, double* d
 #pragma unroll
     for (int k = 0; k < N; k++) a[k] = MADD(sj, Jr[k], a[k]);
   }
-#if TN_FACTOR_VARIANT == 0
 #pragma unroll
   for (int j = 0; j < N; j++) {
     double* cb = colbuf + (j & 1) * 32;      // double-buffered: one __syncwarp per column is enough
@@ -789,41 +689,6 @@ __device__ __noinline__ void tn_factor(const double* Msrc, double* Lm, double* d
     }
     if (k < N) a[k] = MADD(-cc, cb[k], a[k]);
   }
-#else
-  // Software-pipelined right-looking elimination. The dependent chain of a column is
-  //   a[j] update -> pivot broadcast (shuffle) -> 1/sqrt -> scale -> first update of column j+1,
-  // and a warp issues in order: so the chain of column j+1 is started BEFORE the remaining N-j-2 independent updates
-  // of column j are issued, and those fill its latency. The column itself travels through a double-buffered shared
-  // row: iteration j reads buffer j&1 and publishes column j+1 into the other one, whose last readers (iteration j-1)
-  // are behind the __syncwarp that closed that iteration.
-  double piv = __shfl_sync(FULL, a[0], 0);
-  colbuf[lane] = a[0];
-  double inv = pos_rsqrt(piv < BMJ_MINVAL ? BMJ_MINVAL : piv);
-  __syncwarp();
-#pragma unroll
-  for (int j = 0; j < N; j++) {
-    const double* cb = colbuf + (j & 1) * 32;
-    const double lj = (lane == j ? (piv < BMJ_MINVAL ? BMJ_MINVAL : piv) : a[j]) * inv;      // L[i][j]; the diagonal is sqrt(piv)
-    const double cc = a[j] * (inv * inv);                  // raw_i / piv : a[i][k] -= raw_i raw_k / piv
-    a[j] = lj;
-    if (lane == j) dinv[j] = inv;
-    if (j + 1 < N) {
-      a[j + 1] -= cc * cb[j + 1];
-      piv = __shfl_sync(FULL, a[j + 1], j + 1);            // next pivot: start its chain now
-      colbuf[((j + 1) & 1) * 32 + lane] = a[j + 1];        // raw column j+1 (lanes <= j hold junk that nobody reads)
-      inv = pos_rsqrt(piv < BMJ_MINVAL ? BMJ_MINVAL : piv);
-    }
-    int k = j + 2;
-    if (k < N && (k & 1)) { a[k] -= cc * cb[k]; k++; }
-#pragma unroll
-    for (; k + 1 < N; k += 2) {
-      const double2 s2 = *reinterpret_cast<const double2*>(cb + k);
-      a[k] -= cc * s2.x; a[k + 1] -= cc * s2.y;
-    }
-    if (k < N) a[k] -= cc * cb[k];
-    __syncwarp();
-  }
-#endif
   if (isrow) {
 #pragma unroll
     for (int k = 0; k < N; k++) if (k <= lane) Lm[ti + k] = a[k];
@@ -2018,13 +1883,7 @@ __device__ __forceinline__ void fwd_acceleration(const Ctx& c, const b200mj_io& 
     tn_factor<NVT>(W(M), W(H), W(dinv), lane, W(smooth), W(qaccs), W(J), W(efcSD), reinterpret_cast<const int*>(W(actlist)), opaque_zero(), W(colbuf));
     tn_back<NVT>(W(H), W(dinv), W(qaccs), W(qaccs), lane, 0);
   } else {
-    if (c.L.sparse) {
-      copy_row(W(H), c.Mc, tri(nv), lane);
-      FOR_LANES(i, nv) W(qaccs)[i] = W(smooth)[i];
-      __syncwarp();
-      ldl_factor(m, W(H), W(dinv), nv, lane);
-      ldl_solve(m, W(H), W(dinv), W(qaccs), nv, lane);
-    } else if (c.L.dual) {
+    if (c.L.dual) {
       chol_factor(c.Mc, W(H), W(dinv), nv, lane, nullptr, nullptr);      // qacc_smooth: one more right-hand side of dual_prepare's substitution pass
     } else {
       chol_factor(c.Mc, W(H), W(dinv), nv, lane, W(smooth), W(qaccs));
@@ -2099,11 +1958,7 @@ __device__ __forceinline__ Primal constraint_update(const Ctx& c, int nefc) {
 __device__ __forceinline__ void dual_prepare(const Ctx& c, int nefc) {
   const DevModel& m = c.m; int lane = c.lane; int nv = m.nv, ld = m.ldv;
   const double* Jsrc = c.L.jalias ? c.Jg : W(J);
-  if (c.L.sparse) {                                                      // H holds the factor of M (fwd_acceleration)
-    copy_row(W(dV), Jsrc, nefc * ld, lane);
-    ldl_solve_multi(m, W(H), W(dinv), W(dV), ld, nefc, nv, lane);
-    __syncwarp();
-  } else chol_solve_multi(W(H), W(dinv), nv, Jsrc, W(dV), ld, nefc, lane, W(smooth), W(qaccs));      // + qacc_smooth (fwd_acceleration left it to this pass)
+  chol_solve_multi(W(H), W(dinv), nv, Jsrc, W(dV), ld, nefc, lane, W(smooth), W(qaccs));      // + qacc_smooth (fwd_acceleration left it to this pass)
   if (nefc == 0) return;
   if (c.L.jalias) { copy_row(W(J), c.Jg, nefc * ld, lane); __syncwarp(); }      // over the factor of M, which nothing reads any more
   double* A = W(dS);                                                    // may alias H: chol(M) is dead from here on
@@ -2267,8 +2122,9 @@ __device__ __forceinline__ double line_search(const Ctx& c, int nefc, const Prim
 
 // CTA-wide phase alignment: all warps of a CTA run the same code region at the same time so that instruction
 // lines are fetched from L2 once per CTA, not once per warp (the pass footprint is ~5x the 32 KB L1.5 I-cache).
-// level 1: coarse points (pass start, before / after the solver); 2: every stage boundary; 3: also every Newton trip
-#define PHASE_SYNC(level) do { if (c.sync_level >= (level)) __syncthreads(); } while (0)
+// The fused and position kernels take these barriers at coarse points (pass start, stage boundaries around the solver)
+// whenever a CTA holds more than one warp.
+#define PHASE_SYNC() do { if (blockDim.x > 32) __syncthreads(); } while (0)
 
 template <int NVT>
 __device__ __forceinline__ int solve_newton(const Ctx& c, int nefc) {
@@ -2314,7 +2170,7 @@ __device__ __forceinline__ int solve_newton(const Ctx& c, int nefc) {
   double oldcost = 0;
   while (true) {
     // every warp of the CTA takes the same number of trips: finished environments idle at the barrier
-    if (c.sync_level >= 3) { if (!__syncthreads_or(!done)) break; } else if (done) break;
+    if (c.newton_sync) { if (!__syncthreads_or(!done)) break; } else if (done) break;
     if (!done) {
       const double gnorm = newton_gradient(c);
       bool stop = false;
@@ -2660,13 +2516,8 @@ __device__ __forceinline__ void euler_step(const Ctx& c, double* time) {
     __syncwarp();
     FOR_LANES(i, nv) W(H)[tri(i) + i] += h * m.dof_damping[i];
     __syncwarp();
-    if (c.L.sparse) {
-      ldl_factor(m, W(H), W(dinv), nv, lane);
-      ldl_solve(m, W(H), W(dinv), W(tmpv), nv, lane);
-    } else {
-      chol_factor(W(H), W(H), W(dinv), nv, lane, W(tmpv), W(tmpv));
-      chol_back(W(H), W(dinv), W(tmpv), W(tmpv), nv, lane);
-    }
+    chol_factor(W(H), W(H), W(dinv), nv, lane, W(tmpv), W(tmpv));
+    chol_back(W(H), W(dinv), W(tmpv), W(tmpv), nv, lane);
     FOR_LANES(i, nv) W(qvel)[i] += h * W(tmpv)[i];
   } else FOR_LANES(i, nv) W(qvel)[i] += h * W(qacc)[i];
   FOR_LANES(i, nv) W(qaccws)[i] = W(qacc)[i];
@@ -2731,7 +2582,7 @@ enum { MODE_STEP = 0, MODE_FORWARD = 1 };
 // CVX: as for the position kernels (the primitive-only build shares narrowphase<false> with them, so the two paths stay bit-identical).
 template <bool CVX>
 __device__ __forceinline__ void step_kernel_body(const DevModel& m, const Lay& L, const b200mj_io& io,
-                   int batch, int nstep, int flags, int mode, int extra_disable, int sync_level, const uint8_t* env_mask) {
+                   int batch, int nstep, int flags, int mode, int extra_disable, const uint8_t* env_mask) {
   B200MJ_DYN_SMEM
   int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int env = blockIdx.x * (blockDim.x >> 5) + warp;
@@ -2739,7 +2590,7 @@ __device__ __forceinline__ void step_kernel_body(const DevModel& m, const Lay& L
   // and never store; so do the warps of environments outside env_mask (masked reset / forward)
   const bool live = env < batch && (env_mask == nullptr || env_mask[env < batch ? env : 0] != 0);
   if (env >= batch) env = batch - 1;
-  Ctx c(m, L, smem + (size_t)warp * L.total, lane, m.disableflags | extra_disable, blockDim.x > 32 ? sync_level : 0);
+  Ctx c(m, L, smem + (size_t)warp * L.total, lane, m.disableflags | extra_disable, 0);
   c.set_env(env, io);
   size_t e = (size_t)env;
   // ---- load state ----
@@ -2770,42 +2621,36 @@ __device__ __forceinline__ void step_kernel_body(const DevModel& m, const Lay& L
       if (check_bad(c, W(qvel), m.nv)) { w_badqvel++; reset_state(c, &time); }
     }
     // ---------------- position + velocity stage ----------------
-    PHASE_SYNC(1);
+    PHASE_SYNC();
     kinematics(c);
-    PHASE_SYNC(2);
     com_pos(c);
     crb_and_factor(c);
     int ncon = 0, nefc = 0, niter = 0;
     if (!final_pass || full_final) {
       int wfull = 0, cfull = 0;
-      PHASE_SYNC(2);
       ncon = collision<CVX>(c, &wfull);
-      PHASE_SYNC(2);
       nefc = make_constraint(c, ncon, &cfull);
       w_contactfull += wfull; w_cnstrfull += cfull;
     }
-    PHASE_SYNC(2);
     fwd_velocity(c);
     const bool out_posvel = final_pass || forward || (!legacy && last && sub == 0);
     if (out_posvel) subtree_vel(c);
     // ---------------- acceleration stage ----------------
     if (!final_pass) {
-      PHASE_SYNC(2);
       fwd_actuation(c);
       fwd_acceleration<0>(c, io, env);
-      PHASE_SYNC(1);
+      PHASE_SYNC();
       niter = m.solver == BMJ_SOL_PGS ? solve_pgs(c, nefc) : solve_newton<0>(c, nefc);
     }
     if (sub == 0) { r_ncon = ncon; r_nefc = nefc; if (!final_pass) r_niter = niter; }
     const bool out_acc = !final_pass && sub == 0 && last;
     const int smask = want_sens ? ((out_posvel ? 3 : 0) | (out_acc ? 4 : 0)) : 0;
-    PHASE_SYNC(1);
+    PHASE_SYNC();
     if ((smask & 4) && m.acc_sensors) rne_post_constraint(c, io, env, ncon);
     if (smask) sensors(c, smask, ncon);
     if (live && (out_posvel || out_acc)) write_outputs(c, io, env, r_ncon, r_nefc, r_niter, out_posvel, out_acc, want_sens && out_posvel);
     if (final_pass || forward) break;
     // ---------------- integration ----------------
-    PHASE_SYNC(2);
     if (sub == 0 && check_bad(c, W(qacc), m.nv)) { w_badqacc++; reset_state(c, &time); step_idx++; continue; }
     if (!rk4) { euler_step<0>(c, &time); step_idx++; }
     else {
@@ -2856,13 +2701,13 @@ __device__ __forceinline__ void step_kernel_body(const DevModel& m, const Lay& L
 }
 extern "C" __global__ void __launch_bounds__(256)
 b200mj_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ b200mj_io io,
-                   int batch, int nstep, int flags, int mode, int extra_disable, int sync_level, const uint8_t* env_mask) {
-  step_kernel_body<true>(m, L, io, batch, nstep, flags, mode, extra_disable, sync_level, env_mask);
+                   int batch, int nstep, int flags, int mode, int extra_disable, const uint8_t* env_mask) {
+  step_kernel_body<true>(m, L, io, batch, nstep, flags, mode, extra_disable, env_mask);
 }
 extern "C" __global__ void __launch_bounds__(256)
 b200mj_step_prim_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ b200mj_io io,
-                        int batch, int nstep, int flags, int mode, int extra_disable, int sync_level, const uint8_t* env_mask) {
-  step_kernel_body<false>(m, L, io, batch, nstep, flags, mode, extra_disable, sync_level, env_mask);
+                        int batch, int nstep, int flags, int mode, int extra_disable, const uint8_t* env_mask) {
+  step_kernel_body<false>(m, L, io, batch, nstep, flags, mode, extra_disable, env_mask);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2887,7 +2732,7 @@ __device__ __forceinline__ void pos_kernel_body(const DevModel& m, const Lay& L,
   // rewrite identical values and skip the warning counters.
   const bool live = env < batch;
   if (!live) env = batch - 1;
-  Ctx c(m, L, smem + (size_t)warp * L.total, lane, m.disableflags | extra_disable, blockDim.x > 32 ? 1 : 0);
+  Ctx c(m, L, smem + (size_t)warp * L.total, lane, m.disableflags | extra_disable, 0);
   c.set_env(env, io);
   size_t e = (size_t)env;
   // A shadow warp gets a handover row of its own: the stages read back what they wrote there (raw-contact staging, Jacobian rows), so
@@ -2911,20 +2756,20 @@ __device__ __forceinline__ void pos_kernel_body(const DevModel& m, const Lay& L,
     if (io.time && lane == 0) io.time[e] = 0;
     __syncwarp();
   }
-  PHASE_SYNC(1);
+  PHASE_SYNC();
   kinematics(c);
   int wfull = 0, cfull = 0, ncon = 0, nefc = 0;
   const bool with_constraints = !FINAL || (flags & B200MJ_STEP_FULL_FINAL) != 0;
-  PHASE_SYNC(1);
+  PHASE_SYNC();
   if (with_constraints) ncon = collision<CVX>(c, &wfull);   // before com_pos: staging lives in the block com_pos starts to fill
-  PHASE_SYNC(1);
+  PHASE_SYNC();
   com_pos(c);
   crb_and_factor(c);
-  PHASE_SYNC(1);
+  PHASE_SYNC();
   if (with_constraints) nefc = make_constraint(c, ncon, &cfull);
-  PHASE_SYNC(1);
+  PHASE_SYNC();
   fwd_velocity(c);
-  PHASE_SYNC(1);
+  PHASE_SYNC();
   if (FINAL) {
     // (the sensor block shares storage with cacc / cfrc, which fwd_velocity has finished with; the acceleration-stage values of the last physics step are kept)
     if (io.sensordata) FOR_LANES(i, m.nsensordata) W(sens)[i] = io.sensordata[e * m.nsensordata + i];
@@ -2948,25 +2793,21 @@ __device__ __forceinline__ void pos_kernel_body(const DevModel& m, const Lay& L,
     }
   }
   FOR_LANES(i, m.nq) io.qpos[e * m.nq + i] = W(qpos)[i];      // quaternions were normalised in place
-  if (cp.count != nullptr && (!FINAL || with_constraints)) {
+  if (!FINAL || with_constraints) {
     // bucket lists for the acceleration launches: one shared-memory ticket per environment, one global atomic per CTA
     // and bucket (every warp of the CTA gets here: the shadows of environments past the batch end take no ticket)
-    int* cta = reinterpret_cast<int*>(smem + (size_t)(blockDim.x >> 5) * L.total);      // 16 ints behind the workspaces
-    if (threadIdx.x < 16) cta[threadIdx.x] = 0;
+    int* cta = reinterpret_cast<int*>(smem + (size_t)(blockDim.x >> 5) * L.total);      // 8 ints behind the workspaces (64 bytes reserved)
+    if (threadIdx.x < 4) cta[threadIdx.x] = 0;
     __syncthreads();
     int b = 0, my = 0;
     if (live && lane == 0) {
       while (b + 1 < cp.nbucket && nefc > cp.rows_cap[b]) b++;
-      if (cp.prev_niter && cp.prev_niter[env] > cp.niter_split) b += 4;      // slow class: from the back of the list
       my = atomicAdd(&cta[b], 1);
     }
     __syncthreads();
-    if (threadIdx.x < 8) cta[8 + threadIdx.x] = cta[threadIdx.x] ? atomicAdd(&cp.count[threadIdx.x], cta[threadIdx.x]) : 0;
+    if (threadIdx.x < 4) cta[4 + threadIdx.x] = cta[threadIdx.x] ? atomicAdd(&cp.count[threadIdx.x], cta[threadIdx.x]) : 0;
     __syncthreads();
-    if (live && lane == 0) {
-      const int at = cta[8 + b] + my;
-      cp.list[(size_t)(b & 3) * cp.cap + (b < 4 ? at : cp.cap - 1 - at)] = env;
-    }
+    if (live && lane == 0) cp.list[(size_t)b * cp.cap + cta[4 + b] + my] = env;
   }
   if (live && io.warning && lane == 0) {
     int* w = io.warning + e * BMJ_NWARNING;
@@ -3025,43 +2866,28 @@ b200mj_posfinal_prim_kernel(const __grid_constant__ DevModel m, const __grid_con
 // LAST = last physics step of a fused step(): acceleration-stage sensors and outputs are produced here
 template <bool LAST, int NVT>
 __device__ __forceinline__ void acc_kernel_body(const DevModel& m, const Lay& L, const Hand& H, const Hand2& H2, const b200mj_io& io,
-                                                const double* hand, const double* hand2, int batch, int extra_disable, int first_pass,
-                                                int rows_gt, int rows_le, int flags, int env0, const int* bucket_count, const int* bucket_list,
-                                                int list_cap, int* niter_out) {
+                                                const double* hand, const double* hand2, int extra_disable, int first_pass, int flags,
+                                                const int* bucket_count, const int* bucket_list) {
   B200MJ_DYN_SMEM
   int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int env;
+  // One launch per row-count bucket: the CTAs walk the bucket's environment list (*bucket_count entries), which the
+  // position kernel filled. The warps of a multi-warp CTA are phase-aligned by barriers (load -> M^-1 -> every Newton
+  // trip -> Euler), so that instruction lines are fetched once per CTA: the unrolled algebra executes 83 KB of SASS
+  // against a 32 KB L1.5 I-cache. Warps past the end of the list then shadow its last entry (same control flow, no stores).
+  const bool sync = blockDim.x > 32;
+  const int n = bucket_count[0];
+  int k = blockIdx.x * (blockDim.x >> 5) + warp;
   bool live = true;
-  // B200MJ_ACC_SYNC: the warps of a compacted CTA are phase-aligned by barriers (load -> M^-1 -> every Newton trip ->
-  // Euler), so that instruction lines are fetched once per CTA: the unrolled algebra executes 83 KB of SASS against a
-  // 32 KB L1.5 I-cache. Warps past the end of the list then shadow its last entry (same control flow, no stores).
-  const bool sync = (flags & B200MJ_INTERNAL_ACC_SYNC) != 0 && bucket_list != nullptr && blockDim.x > 32;
-  if (bucket_list != nullptr) {
-    // compacted launch: the first CTAs walk the bucket's fast class from the front of its list, the following ones the
-    // slow class from the back (bucket_count[0], bucket_count[4]: entries of either class; list_cap = list length)
-    const int W = blockDim.x >> 5;
-    const int n0 = bucket_count[0], n1 = bucket_count[4], c0 = (n0 + W - 1) / W;
-    int cta_id = blockIdx.x, n = n0;
-    const bool slow = cta_id >= c0;
-    if (slow) { cta_id -= c0; n = n1; }
-    int k = cta_id * W + warp;
-    if (k >= n) {
-      if (!sync || cta_id * W >= n) return;
-      live = false; k = n - 1;
-    }
-    env = bucket_list[slow ? list_cap - 1 - k : k];
-  } else {
-    env = env0 + blockIdx.x * (blockDim.x >> 5) + warp;
-    if (env >= batch) return;
+  if (k >= n) {
+    if (!sync || blockIdx.x * (blockDim.x >> 5) >= n) return;
+    live = false; k = n - 1;
   }
+  const int env = bucket_list[k];
   size_t e = (size_t)env;
   const double* hrow = hand + e * H.total;
   const int* cnt = reinterpret_cast<const int*>(hrow + H.counts);
   const int ncon = cnt[0], nefc = cnt[1];
-  // row-count bucket: this launch's workspace holds up to rows_le constraint rows; environments with more (or
-  // fewer than rows_gt+1) rows are served by the launch with the matching workspace and leave at once here
-  if (!sync && (nefc <= rows_gt || nefc > rows_le)) return;
-  Ctx c(m, L, smem + (size_t)warp * L.total, lane, m.disableflags | extra_disable, sync ? ((flags & B200MJ_INTERNAL_ACC_SYNC_COARSE) ? 1 : 3) : 0);
+  Ctx c(m, L, smem + (size_t)warp * L.total, lane, m.disableflags | extra_disable, sync);
   c.set_env(env, io);
   const int nv = NVT > 0 ? NVT : m.nv, ld = NVT > 0 ? (NVT | 1) : m.ldv;
   // ---- load state + handover ----
@@ -3095,7 +2921,6 @@ __device__ __forceinline__ void acc_kernel_body(const DevModel& m, const Lay& L,
   if (check_bad(c, W(qacc), nv)) { w_badqacc = 1; reset_state(c, &time); }
   else euler_step<NVT>(c, &time);
   if (!live) return;      // shadows: no stores (the sensor epilogue below has no barriers)
-  if (niter_out && lane == 0) niter_out[env] = niter;      // the next physics step's CTA class
   // ---- store state ----
   FOR_LANES(i, m.nq) io.qpos[e * m.nq + i] = W(qpos)[i];
   FOR_LANES(i, nv) { io.qvel[e * nv + i] = W(qvel)[i]; if (io.qacc_warmstart) io.qacc_warmstart[e * nv + i] = W(qaccws)[i]; }
@@ -3129,31 +2954,26 @@ __device__ __forceinline__ void acc_kernel_body(const DevModel& m, const Lay& L,
 extern "C" __global__ void __launch_bounds__(256)
 b200mj_acc_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Hand H,
                   const __grid_constant__ Hand2 H2, const __grid_constant__ b200mj_io io, const double* hand, const double* hand2,
-                  int batch, int extra_disable, int first_pass, int rows_gt, int rows_le, int flags, int env0, const int* bucket_count,
-                  const int* bucket_list, int list_cap, int* niter_out) {
-  acc_kernel_body<false, 0>(m, L, H, H2, io, hand, hand2, batch, extra_disable, first_pass, rows_gt, rows_le, flags, env0, bucket_count, bucket_list, list_cap, niter_out);
+                  int extra_disable, int first_pass, int flags, const int* bucket_count, const int* bucket_list) {
+  acc_kernel_body<false, 0>(m, L, H, H2, io, hand, hand2, extra_disable, first_pass, flags, bucket_count, bucket_list);
 }
 extern "C" __global__ void __launch_bounds__(256)
 b200mj_acclast_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Hand H,
                       const __grid_constant__ Hand2 H2, const __grid_constant__ b200mj_io io, const double* hand, const double* hand2,
-                  int batch, int extra_disable, int first_pass, int rows_gt, int rows_le, int flags, int env0, const int* bucket_count,
-                  const int* bucket_list, int list_cap, int* niter_out) {
-  acc_kernel_body<true, 0>(m, L, H, H2, io, hand, hand2, batch, extra_disable, first_pass, rows_gt, rows_le, flags, env0, bucket_count, bucket_list, list_cap, niter_out);
+                  int extra_disable, int first_pass, int flags, const int* bucket_count, const int* bucket_list) {
+  acc_kernel_body<true, 0>(m, L, H, H2, io, hand, hand2, extra_disable, first_pass, flags, bucket_count, bucket_list);
 }
 
 // Acceleration kernels with nv fixed at compile time (register-resident algebra, tn_* above). One instantiation per
 // nv of B200MJ_NV_LIST — the dofs of the benchmark configurations (cheetah 9, quadruped 22, humanoid 27) and a few
 // common small sizes; any other model runs the runtime-size kernels above. Same arguments, same handover format.
-#ifndef B200MJ_NV_LIST
 #define B200MJ_NV_LIST(X) X(6) X(9) X(12) X(18) X(22) X(27)
-#endif
 template <bool LAST, int NVT>
 __global__ void __launch_bounds__(128, 4)
 b200mj_acc_tn_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Hand H,
                      const __grid_constant__ Hand2 H2, const __grid_constant__ b200mj_io io, const double* hand, const double* hand2,
-                     int batch, int extra_disable, int first_pass, int rows_gt, int rows_le, int flags, int env0, const int* bucket_count,
-                     const int* bucket_list, int list_cap, int* niter_out) {
-  acc_kernel_body<LAST, NVT>(m, L, H, H2, io, hand, hand2, batch, extra_disable, first_pass, rows_gt, rows_le, flags, env0, bucket_count, bucket_list, list_cap, niter_out);
+                     int extra_disable, int first_pass, int flags, const int* bucket_count, const int* bucket_list) {
+  acc_kernel_body<LAST, NVT>(m, L, H, H2, io, hand, hand2, extra_disable, first_pass, flags, bucket_count, bucket_list);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -3162,19 +2982,47 @@ b200mj_acc_tn_kernel(const __grid_constant__ DevModel m, const __grid_constant__
 static int64_t g_launches = 0;
 
 typedef void (*acc_kernel_fn)(const DevModel, const Lay, const Hand, const Hand2, const b200mj_io, const double*, const double*,
-                              int, int, int, int, int, int, int, const int*, const int*, int, int*);
-#define BCOUNT_SLOTS 64
-// the compile-time-size acceleration kernel for nv dofs, or nullptr (B200MJ_TN=0 disables them: A/B runs)
+                              int, int, int, const int*, const int*);
+// the compile-time-size acceleration kernel for nv dofs, or nullptr
 static acc_kernel_fn tn_kernel(int nv, bool last) {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("B200MJ_TN"); on = e ? atoi(e) : 1; }
-  if (!on) return nullptr;
   switch (nv) {
 #define TN_CASE(n) case n: return last ? (acc_kernel_fn)b200mj_acc_tn_kernel<true, n> : (acc_kernel_fn)b200mj_acc_tn_kernel<false, n>;
     B200MJ_NV_LIST(TN_CASE)
 #undef TN_CASE
     default: return nullptr;
   }
+}
+
+// Environment overrides, read once per model. Each is a test hook that steers a model onto a path it would not take by
+// itself; unset, the engine makes every one of these choices from the model:
+//   B200MJ_TN=0              runtime-size acceleration kernels although a compile-time-size one exists (the fused,
+//                            split and TN comparisons of test_emu_kernel_parity.py, test_gpu_engine.py and test_dual_newton.py)
+//   B200MJ_SPLIT=0           the fused kernel only (test_launch_knobs_do_not_change_results,
+//                            test_fused_and_split_paths_agree_bitwise)
+//   B200MJ_DUAL_MIN_NV=n     dual Newton direction from n dofs on (default 32; 0: never), forced onto the 27-dof humanoid
+//                            by test_dual_newton.py
+//   B200MJ_CVX_WARP=0        one convex pair per lane (cvx_pair), the bitwise reference for cvx_pair_warp
+//                            (test_engine_convex_contacts_equal_the_oracles_bitwise, test_launch_knobs_do_not_change_results)
+//   B200MJ_BUCKETS=a,b[,c]   acceleration row-bucket capacities below njmax
+//   B200MJ_EPB_POS=n         warps per position-kernel CTA
+//   B200MJ_ACC_WARPS=n       warps per compile-time-size acceleration CTA, at most 4 (default 4)
+//   B200MJ_ENVS_PER_BLOCK=n  warps per fused-kernel CTA
+//                            (these four: launch invariance, test_launch_knobs_do_not_change_results)
+static void read_test_hooks(b200mj_model* M) {
+  auto num = [](const char* name, int dflt) { const char* e = getenv(name); return e ? atoi(e) : dflt; };
+  M->hooks.tn = num("B200MJ_TN", 1);
+  M->hooks.split = num("B200MJ_SPLIT", 1);
+  M->hooks.dual_min_nv = num("B200MJ_DUAL_MIN_NV", 32);
+  M->dm.cvx_warp = num("B200MJ_CVX_WARP", 1);
+  M->hooks.nbuckets = 0;
+  if (const char* e = getenv("B200MJ_BUCKETS")) {
+    const int got = sscanf(e, "%d,%d,%d", &M->hooks.buckets[0], &M->hooks.buckets[1], &M->hooks.buckets[2]);
+    if (got >= 2) M->hooks.nbuckets = got;
+  }
+  M->hooks.epb_pos = num("B200MJ_EPB_POS", 0);
+  M->hooks.acc_warps = num("B200MJ_ACC_WARPS", 4);
+  if (M->hooks.acc_warps < 1 || M->hooks.acc_warps > 8) M->hooks.acc_warps = 4;
+  M->hooks.envs_per_block = num("B200MJ_ENVS_PER_BLOCK", 0);
 }
 
 static void build_layout(b200mj_model* M) {
@@ -3214,7 +3062,7 @@ static void build_layout(b200mj_model* M) {
   // warps of a CTA are phase-aligned with barriers and so share their instruction fetches.
   int best = (int)((227 * 1024) / (M->smem_per_env ? M->smem_per_env : 1));
   if (best > 8) best = 8;
-  if (const char* ev = getenv("B200MJ_ENVS_PER_BLOCK")) { int v = atoi(ev); if (v >= 1 && v <= best) best = v; }
+  if (M->hooks.envs_per_block >= 1 && M->hooks.envs_per_block <= best) best = M->hooks.envs_per_block;
   M->envs_per_block = best;
 
   // ---- split kernels: compact layouts + handover rows ----
@@ -3255,19 +3103,10 @@ static void build_layout(b200mj_model* M) {
     P.grb = take(P.gcache ? m.ngeom : 0); P.gmg = take(P.gcache ? m.ngeom : 0); P.gty = take(P.gcache ? (m.ngeom + 1) / 2 : 0);
     P.total = o;
     M->smem_pos = (size_t)o * sizeof(double);
-    // dual form of the Newton direction in the runtime-size kernels (B200MJ_DUAL_MIN_NV, default 32: the two-rows-per-lane
-    // factorisation; 0 disables)
-    int dual_min_nv = 32;
-    if (const char* ev = getenv("B200MJ_DUAL_MIN_NV")) dual_min_nv = atoi(ev);
+    // dual form of the Newton direction in the runtime-size kernels from dual_min_nv dofs on (32: the two-rows-per-lane
+    // factorisation)
+    const int dual_min_nv = M->hooks.dual_min_nv;
     auto tri_host = [](int i) { return (i * (i + 1)) / 2; };
-    // B200MJ_SPARSE_LDL=1: tree-sparse L'DL for M and M + h B (ldl_factor). OFF by default: measured SLOWER on the CMU corridor
-    // configuration than the blocked dense factorisation although it executes a third of the
-    // multiply-adds — the kernel is bound by per-warp latency (1.5 warps per scheduler), and 62 dependent elimination steps of
-    // a few instructions each are a longer chain than 16 dense column blocks with eight independent accumulators.
-    int mglobal_on = 1, sparse_on = 0, jalias_on = 1;
-    if (const char* ev = getenv("B200MJ_J_ALIAS")) jalias_on = atoi(ev);
-    if (const char* ev = getenv("B200MJ_M_GLOBAL")) mglobal_on = atoi(ev);
-    if (const char* ev = getenv("B200MJ_SPARSE_LDL")) sparse_on = atoi(ev);
     auto acc_layout = [&](Lay& A, int rows, bool with_sens) {
       memset(&A, 0, sizeof(A));
       o = 0;
@@ -3277,13 +3116,12 @@ static void build_layout(b200mj_model* M) {
       // Everything below is dead once the state has been integrated; the sensor-carrying variant then re-uses the
       // storage for the position-stage dump that rne_post_constraint and the acceleration-stage sensors read.
       const int u0 = o;
-      A.mglobal = (mglobal_on && !M->tn_nv && nv >= 32) ? 1 : 0;
-      A.sparse = (A.mglobal && sparse_on && m.dof_anc_adr) ? 1 : 0;
+      A.mglobal = (!M->tn_nv && nv >= 32) ? 1 : 0;
       A.M = take(A.mglobal ? 0 : ntri); A.H = take(ntri); A.dinv = take(nv);
       // dual form with few rows: J's workspace copy aliases H (dual_prepare), so that seven CMU environments fit an SM
       const bool will_dual = dual_min_nv > 0 && !M->tn_nv && nv >= dual_min_nv && rows <= 32 && m.solver == BMJ_SOL_NEWTON;
       const int dneed = rows * rows + tri_host(rows) + 3 * rows + 2;
-      A.jalias = (will_dual && jalias_on && rows * ld + dneed <= ntri) ? 1 : 0;
+      A.jalias = (will_dual && rows * ld + dneed <= ntri) ? 1 : 0;
       A.J = A.jalias ? A.H : take(rows * ld); A.efcD = take(rows); A.efcSD = take(rows); A.aref = take(rows); A.jar = take(rows); A.jv = take(rows);
       A.eqflag = take((rows + 1) / 2); A.actlist = take((rows + 1) / 2);
       A.bias = take(nv); A.passive = take(nv); A.qfact = take(nv); A.smooth = take(nv); A.qaccs = take(nv);
@@ -3305,20 +3143,18 @@ static void build_layout(b200mj_model* M) {
       A.total = o;
       return (size_t)o * sizeof(double);
     };
-    M->smem_acc = acc_layout(M->lay_acc, nj, false);
     // row-count buckets: most environments carry far fewer rows than njmax (humanoid: mean 10, max 43 of 64)
-    // {10, 16, 32, njmax} gave a shorter kernel group than {10, 24, njmax} on the humanoid workload (tools/knob_sweep.sh)
+    // {10, 16, 32, njmax} gave a shorter kernel group than {10, 24, njmax} on the humanoid workload
     int caps[4] = {10, 16, 32, nj};
     int ncap = 4;
     // large capacities (CMU corridor, njmax 200; 91 % of the environments carry <= 12 rows, 99.6 % <= 32): every populated bucket launch
-    // costs one per-environment latency and the launches cannot share SMs (shared memory), so three buckets beat four
-    // (measured per control step with tools/cmu_knobs.sh)
+    // costs one per-environment latency and the launches cannot share SMs (shared memory), so three buckets measured
+    // faster per control step than four
     if (nj > 96) { caps[0] = 12; caps[1] = 32; caps[2] = nj; ncap = 3; }
-    if (const char* ev = getenv("B200MJ_BUCKETS")) {
-      int a1 = 0, a2 = 0, a3 = 0;
-      int got = sscanf(ev, "%d,%d,%d", &a1, &a2, &a3);
-      if (got == 2) { caps[0] = a1; caps[1] = a2; caps[2] = nj; ncap = 3; }
-      else if (got == 3) { caps[0] = a1; caps[1] = a2; caps[2] = a3; caps[3] = nj; ncap = 4; }
+    if (M->hooks.nbuckets) {
+      ncap = M->hooks.nbuckets + 1;
+      for (int k = 0; k < M->hooks.nbuckets; k++) caps[k] = M->hooks.buckets[k];
+      caps[ncap - 1] = nj;
     }
     M->nbucket = 0;
     for (int k = 0; k < ncap; k++) {
@@ -3348,8 +3184,8 @@ static void build_layout(b200mj_model* M) {
     // one 5-warp CTA per SM and room for more warps: the `big` kernels (up to 7 warps, __launch_bounds__(224, 1))
     M->pos_big = 0;
     if (2 * 5 * M->smem_pos + 2 * 64 > 227 * 1024 && pick(M->smem_pos) > 5) { M->pos_big = 1; M->epb_pos = pick(M->smem_pos) > 7 ? 7 : pick(M->smem_pos); }
-    if (const char* ev = getenv("B200MJ_EPB_POS")) { int v = atoi(ev); if (v >= 1 && v <= pick(M->smem_pos) && v <= (M->pos_big ? 7 : 5)) M->epb_pos = v; }   // __launch_bounds__(160, ..)
-    M->epb_acc = pick(M->smem_accs_b[M->nbucket - 1]) >= 1 ? 1 : 0;   // one warp per CTA: out-of-bucket environments exit at once
+    const int v = M->hooks.epb_pos;
+    if (v >= 1 && v <= pick(M->smem_pos) && v <= (M->pos_big ? 7 : 5)) M->epb_pos = v;   // __launch_bounds__(160, ..)
   }
 }
 
@@ -3475,7 +3311,6 @@ int b200mj_model_create(const int32_t* idata, int ni, const double* rdata, int n
                             (t1 == BMJ_GEOM_CAPSULE && t2 == BMJ_GEOM_CAPSULE);
       if (!analytic) M->convex_pairs = 1;
     }
-    if (const char* ev = getenv("B200MJ_POS_CVX")) if (atoi(ev) == 1) M->convex_pairs = 1;   // A/B: force the general build
     const int nv = m.nv, nu = m.nu;
     int* adr = new int[nv + 1];
     int* ids = new int[(size_t)nv * (nu > 0 ? nu : 1)];
@@ -3499,46 +3334,21 @@ int b200mj_model_create(const int32_t* idata, int ni, const double* rdata, int n
     }
     adr[nv] = n;
     const int nn = n > 0 ? n : 1;
-    // dof tree tables (ldl_factor / ldl_solve): ancestor lists, subtree sizes; valid when dofs are numbered depth-first
-    // (parent before child, subtrees contiguous), which the compiler guarantees — checked here, else the dense path stays
-    int* aadr = new int[nv + 1];
-    int* aid = new int[(size_t)nv * (nv > 0 ? nv : 1) / 2 + 1];
-    int* sub = new int[nv > 0 ? nv : 1];
-    int na = 0; bool tree_ok = true;
-    for (int k = 0; k < nv; k++) {
-      aadr[k] = na;
-      for (int i = hf.dof_parentid[k]; i >= 0; i = hf.dof_parentid[i]) { if (i >= k) { tree_ok = false; break; } aid[na++] = i; }
-      if (!tree_ok) break;
-      sub[k] = 1;
-    }
-    aadr[nv] = na;
-    if (tree_ok) {
-      for (int k = nv - 1; k >= 0; k--) if (hf.dof_parentid[k] >= 0) sub[hf.dof_parentid[k]] += sub[k];
-      for (int k = 0; k < nv && tree_ok; k++)      // contiguity: every dof in (k, k + sub[k]) must descend from k
-        for (int q = k + 1; q < k + sub[k]; q++) { int i = q; while (i > k) i = hf.dof_parentid[i]; if (i != k) { tree_ok = false; break; } }
-    }
-    const int naa = na > 0 ? na : 1;
-    bool ok = cudaMalloc(&M->d_xi, (size_t)(nv + 1 + nn + (nv + 1) + naa + (nv > 0 ? nv : 1)) * sizeof(int)) == cudaSuccess &&
+    bool ok = cudaMalloc(&M->d_xi, (size_t)(nv + 1 + nn) * sizeof(int)) == cudaSuccess &&
               cudaMalloc(&M->d_xr, (size_t)nn * sizeof(double)) == cudaSuccess;
-    int* d_aadr = M->d_xi + nv + 1 + nn; int* d_aid = d_aadr + nv + 1; int* d_sub = d_aid + naa;
     if (ok) ok = cudaMemcpy(M->d_xi, adr, (size_t)(nv + 1) * sizeof(int), cudaMemcpyHostToDevice) == cudaSuccess &&
                  cudaMemcpy(M->d_xi + nv + 1, ids, (size_t)nn * sizeof(int), cudaMemcpyHostToDevice) == cudaSuccess &&
                  cudaMemcpy(M->d_xr, coef, (size_t)nn * sizeof(double), cudaMemcpyHostToDevice) == cudaSuccess;
-    if (ok && tree_ok && nv > 0) ok = cudaMemcpy(d_aadr, aadr, (size_t)(nv + 1) * sizeof(int), cudaMemcpyHostToDevice) == cudaSuccess &&
-                 cudaMemcpy(d_aid, aid, (size_t)naa * sizeof(int), cudaMemcpyHostToDevice) == cudaSuccess &&
-                 cudaMemcpy(d_sub, sub, (size_t)nv * sizeof(int), cudaMemcpyHostToDevice) == cudaSuccess;
-    delete[] adr; delete[] ids; delete[] coef; delete[] aadr; delete[] aid; delete[] sub;
+    delete[] adr; delete[] ids; delete[] coef;
     if (!ok) { b200mj_model_destroy(M); return -2; }
     m.dof_act_adr = M->d_xi; m.dof_act_id = M->d_xi + nv + 1; m.dof_act_coef = M->d_xr;
-    if (tree_ok && nv > 0) { m.dof_anc_adr = d_aadr; m.dof_anc_id = d_aid; m.dof_subsize = d_sub; }
-    else { m.dof_anc_adr = nullptr; m.dof_anc_id = nullptr; m.dof_subsize = nullptr; }
   }
-  { const char* ev = getenv("B200MJ_CVX_WARP"); m.cvx_warp = ev ? atoi(ev) : 1; }
+  read_test_hooks(M);
   M->nkey = h_sizes[BMJ_NKEY];
-  M->tn_nv = tn_kernel(m.nv, false) ? m.nv : 0;
+  M->tn_nv = (M->hooks.tn && tn_kernel(m.nv, false)) ? m.nv : 0;
   build_layout(M);
   if (M->envs_per_block < 1) { b200mj_model_destroy(M); return -4; }
-  for (int g = 0; g < 3; g++) {
+  for (int g = 0; g < 2; g++) {
     cudaStreamCreateWithFlags(&M->gmain[g], cudaStreamNonBlocking);
     cudaEventCreateWithFlags(&M->ev_join[g], cudaEventDisableTiming); cudaEventCreateWithFlags(&M->ev_pos[g], cudaEventDisableTiming);
     for (int b = 0; b < 4; b++) { cudaStreamCreateWithFlags(&M->gaux[g][b], cudaStreamNonBlocking); cudaEventCreateWithFlags(&M->ev_acc[g][b], cudaEventDisableTiming); }
@@ -3573,9 +3383,8 @@ void b200mj_model_destroy(b200mj_model* M) {
   if (M->d_hand2) cudaFree(M->d_hand2);
   if (M->d_bcount) cudaFree(M->d_bcount);
   if (M->d_blist) cudaFree(M->d_blist);
-  if (M->d_niter) cudaFree(M->d_niter);
   if (M->streams_ok) {
-    for (int g = 0; g < 3; g++) {
+    for (int g = 0; g < 2; g++) {
       cudaStreamDestroy(M->gmain[g]); cudaEventDestroy(M->ev_join[g]); cudaEventDestroy(M->ev_pos[g]);
       for (int b = 0; b < 4; b++) { cudaStreamDestroy(M->gaux[g][b]); cudaEventDestroy(M->ev_acc[g][b]); }
     }
@@ -3657,19 +3466,10 @@ static int launch(const b200mj_model* M, const b200mj_io* io, int batch, int nst
   if (!io->qpos || !io->qvel || (M->dm.na > 0 && !io->act)) return -1;
   int epb = M->envs_per_block;
   int grid = (batch + epb - 1) / epb;
-  size_t smem = M->smem_per_env * epb;
-  if (const char* pad = getenv("B200MJ_EXTRA_SMEM")) smem += (size_t)atoi(pad);   // occupancy experiments only
-  static int sync_level = -1;
-  if (sync_level < 0) { const char* sl = getenv("B200MJ_SYNC_LEVEL"); sync_level = sl ? atoi(sl) : 1; }
-  B200MJ_LAUNCH((M->convex_pairs ? b200mj_step_kernel : b200mj_step_prim_kernel), grid, 32 * epb, smem, (cudaStream_t)stream, M->dm, M->lay, *io, batch, nstep, flags, mode, extra, sync_level, env_mask);
+  const size_t smem = M->smem_per_env * epb;
+  B200MJ_LAUNCH((M->convex_pairs ? b200mj_step_kernel : b200mj_step_prim_kernel), grid, 32 * epb, smem, (cudaStream_t)stream, M->dm, M->lay, *io, batch, nstep, flags, mode, extra, env_mask);
   g_launches++;
   return cudaGetLastError() == cudaSuccess ? 0 : -5;
-}
-
-static int split_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("B200MJ_SPLIT"); v = e ? atoi(e) : 2; }
-  return v;
 }
 
 int b200mj_step(const b200mj_model* Mc, const b200mj_io* io, int batch, int nstep, int flags, void* stream) {
@@ -3677,10 +3477,10 @@ int b200mj_step(const b200mj_model* Mc, const b200mj_io* io, int batch, int nste
   if (!M || !io || batch <= 0 || nstep < 0) return -1;
   // Split path: Euler, legacy ordering, no applied forces routed in, workspaces fit. Everything else (RK4, the
   // non-legacy ordering, qfrc/xfrc_applied) runs through the fused kernel.
-  bool can_split = split_enabled() && nstep >= (split_enabled() >= 2 ? 1 : 2) && (flags & B200MJ_STEP_LEGACY) && M->dm.integrator == BMJ_INT_EULER &&
+  bool can_split = M->hooks.split && nstep >= 1 && (flags & B200MJ_STEP_LEGACY) && M->dm.integrator == BMJ_INT_EULER &&
                    M->dm.solver == BMJ_SOL_NEWTON &&
-                   !io->qfrc_applied && !io->xfrc_applied && M->epb_pos >= 1 && M->epb_acc >= 1 && io->qpos && io->qvel &&
-                   (M->dm.na == 0 || io->act);
+                   !io->qfrc_applied && !io->xfrc_applied && M->epb_pos >= 1 && M->smem_accs_b[M->nbucket - 1] <= 227 * 1024 &&
+                   io->qpos && io->qvel && (M->dm.na == 0 || io->act);
   if (!can_split) return launch(M, io, batch, nstep, flags, MODE_STEP, 0, stream);
   if (M->hand_batch < batch) {
     if (M->d_hand) cudaFree(M->d_hand);
@@ -3691,134 +3491,89 @@ int b200mj_step(const b200mj_model* Mc, const b200mj_io* io, int batch, int nste
     if (M->d_bcount) cudaFree(M->d_bcount);
     if (M->d_blist) cudaFree(M->d_blist);
     M->d_bcount = M->d_blist = nullptr;
-    if (M->d_niter) cudaFree(M->d_niter);
-    M->d_niter = nullptr;
-    if (cudaMalloc(&M->d_bcount, (size_t)3 * BCOUNT_SLOTS * 8 * sizeof(int)) != cudaSuccess) return -2;
-    if (cudaMalloc(&M->d_blist, (size_t)3 * 4 * batch * sizeof(int)) != cudaSuccess) return -2;
-    if (cudaMalloc(&M->d_niter, (size_t)batch * sizeof(int)) != cudaSuccess) return -2;
-    cudaMemset(M->d_bcount, 0, (size_t)3 * BCOUNT_SLOTS * 8 * sizeof(int));
-    cudaMemset(M->d_niter, 0, (size_t)batch * sizeof(int));
+    if (cudaMalloc(&M->d_bcount, (size_t)2 * 4 * sizeof(int)) != cudaSuccess) return -2;
+    if (cudaMalloc(&M->d_blist, (size_t)2 * 4 * batch * sizeof(int)) != cudaSuccess) return -2;
+    cudaMemset(M->d_bcount, 0, (size_t)2 * 4 * sizeof(int));
     M->hand_batch = batch;
   }
   cudaStream_t st = (cudaStream_t)stream;
   const bool want_sens = (flags & B200MJ_STEP_SENSORS) != 0;
-  // split_enabled() == 2 (default): every physics step split; the last one uses the sensor-carrying acceleration
-  // kernel and the trailing mj_step1 is the `posfinal` kernel (12 % faster than == 1 with concurrent bucket streams).
-  // == 1: split kernels for the first nstep-1 physics steps, the fused kernel for the last one. == 0: fused only.
-  const bool all_split = split_enabled() >= 2;
-  const int nsplit = all_split ? nstep : nstep - 1;
+  // Every physics step is split; the last one uses the sensor-carrying acceleration kernel and the trailing mj_step1 is
+  // the `posfinal` kernel.
   // B200MJ_STEP_REUSE_POS: the previous call's trailing mj_step1 wrote this state's handover rows already
   // (the trailing mj_step1 dumps what the acceleration-stage sensors need only when the call had one physics step: a
   // call whose first step is also its last must then find that dump, or recompute the position stage)
-  const bool reuse = (flags & B200MJ_STEP_REUSE_POS) && all_split && nstep >= 1 && M->reuse_ok && M->reuse_qpos == io->qpos &&
+  const bool reuse = (flags & B200MJ_STEP_REUSE_POS) && M->reuse_ok && M->reuse_qpos == io->qpos &&
                      M->reuse_batch == batch && M->reuse_flags == (flags & ~B200MJ_STEP_REUSE_POS) &&
                      (nstep > 1 || !want_sens || M->reuse_has_dump);
   M->reuse_ok = 0;
-  // Environment groups (B200MJ_GROUPS, default 2 for batches >= 2048): the launch sequence of each group is
-  // independent of the others, so groups run on their own streams and one group's position kernel fills the tail of
-  // the other's acceleration kernels. On the humanoid workload 2 groups measured faster than 1 and 3 (with the earlier,
-  // larger workspaces 2 groups were slower: too few warps of each kind fitted an SM side by side).
-  static int ngroups_env = -1;
-  if (ngroups_env < 0) { const char* e = getenv("B200MJ_GROUPS"); ngroups_env = e ? atoi(e) : 2; if (ngroups_env < 1) ngroups_env = 1; if (ngroups_env > 3) ngroups_env = 3; }
-  int ngroups = (all_split && batch >= 2048) ? ngroups_env : 1;
-  static int acc_pad = -1;    // occupancy experiments only: extra dynamic shared memory per acceleration CTA
-  if (acc_pad < 0) { const char* e = getenv("B200MJ_ACC_PAD"); acc_pad = e ? atoi(e) : 0; }
-  // Row-bucket compaction (B200MJ_COMPACT, default on): acceleration CTAs of B200MJ_ACC_WARPS warps over dense per-bucket
-  // environment lists. Slot k of a group's counters belongs to physics step k of a call; the trailing mj_step1 writes
-  // slot 0 for the next call (B200MJ_STEP_REUSE_POS). The slot sequence is the same in every call, so a captured
-  // CUDA graph of this function stays valid.
+  // Environment groups (2 for batches >= 2048): the launch sequence of each group is independent of the other's, so
+  // groups run on their own streams and one group's position kernel fills the tail of the other's acceleration kernels.
+  // On the humanoid workload 2 groups measured faster than 1 and 3 (with the earlier, larger workspaces 2 groups were
+  // slower: too few warps of each kind fitted an SM side by side).
+  const int ngroups = batch >= 2048 ? 2 : 1;
+  // Row-bucket compaction: acceleration CTAs of several warps over dense per-bucket environment lists. Each group has
+  // one set of bucket counters and lists, refilled by every position launch and read by the acceleration launches of
+  // the same physics step. Reuse across steps is ordered by the group stream: every bucket stream joins back into it
+  // (ev_acc) before the next position launch and its counter reset are queued there. The trailing mj_step1 fills them
+  // for the next call's first acceleration launches (B200MJ_STEP_REUSE_POS). The launch sequence is the same in every
+  // call, so a captured CUDA graph of this function stays valid.
   // On the humanoid workload 4 phase-aligned warps per CTA gave the shortest kernel group of one-warp CTAs and compacted
   // CTAs of 2, 3, 4 and 8 warps. The compile-time-size kernels are built for at most 4 warps per CTA (__launch_bounds__(128, 4)).
-  static int niter_split = 0;      // B200MJ_NITER_SPLIT: iteration count above which an environment joins its bucket's slow class (0: one class)
-  static int compact_on = -1, acc_warps = 4, acc_sync = 2;      // B200MJ_ACC_SYNC: 0 off, 1 stage boundaries only, 2 + every Newton trip
-  if (compact_on < 0) {
-    const char* e = getenv("B200MJ_COMPACT"); compact_on = e ? atoi(e) : 1;
-    if (const char* a = getenv("B200MJ_ACC_SYNC")) acc_sync = atoi(a);
-    if (const char* n = getenv("B200MJ_NITER_SPLIT")) niter_split = atoi(n);
-    if (const char* w = getenv("B200MJ_ACC_WARPS")) { int v = atoi(w); if (v >= 1 && v <= 8) acc_warps = v; }
-  }
-  const bool compact = compact_on && all_split && nstep + 1 <= BCOUNT_SLOTS && M->d_bcount && M->d_blist;
   if (ngroups > 1) cudaEventRecord(M->ev_fork, st);
   for (int g = 0; g < ngroups; g++) {
     const int e0 = (int)((long long)batch * g / ngroups), e1 = (int)((long long)batch * (g + 1) / ngroups), cnt = e1 - e0;
     cudaStream_t sm = (g == 0) ? st : M->gmain[g];
     if (g > 0) cudaStreamWaitEvent(sm, M->ev_fork, 0);
     const int gp = (cnt + M->epb_pos - 1) / M->epb_pos;
-    int* gcount = M->d_bcount ? M->d_bcount + (size_t)g * BCOUNT_SLOTS * 8 : nullptr;
-    int* glist = M->d_blist ? M->d_blist + (size_t)g * 4 * M->hand_batch : nullptr;
-    auto compact_for = [&](int slot) {
+    int* gcount = M->d_bcount + (size_t)g * 4;
+    int* glist = M->d_blist + (size_t)g * 4 * M->hand_batch;
+    auto compact = [&]() {
       Compact cp; memset(&cp, 0, sizeof(cp));
       cp.shadow_row = M->hand_batch + g * 8;
-      if (compact) {
-        cp.count = gcount + slot * 8; cp.list = glist; cp.cap = M->hand_batch; cp.nbucket = M->nbucket;
-        for (int b = 0; b < M->nbucket; b++) cp.rows_cap[b] = M->rows_cap[b];
-        cp.prev_niter = niter_split > 0 ? M->d_niter : nullptr; cp.niter_split = niter_split;
-        cudaMemsetAsync(cp.count, 0, 8 * sizeof(int), sm);
-      }
+      cp.count = gcount; cp.list = glist; cp.cap = M->hand_batch; cp.nbucket = M->nbucket;
+      for (int b = 0; b < M->nbucket; b++) cp.rows_cap[b] = M->rows_cap[b];
+      cudaMemsetAsync(cp.count, 0, 4 * sizeof(int), sm);
       return cp;
     };
-    for (int s = 0; s < nsplit; s++) {
-      const bool last = all_split && s == nstep - 1;
+    for (int s = 0; s < nstep; s++) {
+      const bool last = s == nstep - 1;
       if (!(reuse && s == 0)) {
-        const Compact cp = compact_for(s);
+        const Compact cp = compact();
         B200MJ_LAUNCH((M->pos_big ? b200mj_pos_big_kernel : M->convex_pairs ? b200mj_pos_kernel : b200mj_pos_prim_kernel), gp, 32 * M->epb_pos, M->smem_pos * M->epb_pos + 64, sm, M->dm, M->lay_pos, M->hand, M->hand2, *io, M->d_hand, M->d_hand2,
                                                                                  e1, 0, flags, last && want_sens, e0, cp);
         g_launches++;
       }
       if (M->nbucket > 1) cudaEventRecord(M->ev_pos[g], sm);
-      // optional largest-rows-first launch order: the big-workspace environments run longest, so they could start earliest and the
-      // many small ones fill in around them (B200MJ_BUCKET_ORDER=1; measured equal to ascending order on the humanoid workload, so ascending stays the default)
-      static int desc = -1;
-      if (desc < 0) { const char* e = getenv("B200MJ_BUCKET_ORDER"); desc = e ? atoi(e) : 0; }
-      for (int bb = 0; bb < M->nbucket; bb++) {
-        const int b = desc ? M->nbucket - 1 - bb : bb;
-        int gt = b == 0 ? -1 : M->rows_cap[b - 1], le = M->rows_cap[b];
+      for (int b = 0; b < M->nbucket; b++) {
         cudaStream_t sb = b == 0 ? sm : M->gaux[g][b];     // buckets are independent: let them share the SMs
         if (b > 0) cudaStreamWaitEvent(sb, M->ev_pos[g], 0);
         const size_t ws = (last ? M->smem_accs_b[b] : M->smem_acc_b[b]);
-        // warps per CTA of a compacted launch: as many as fit 227 KB, at most acc_warps
-        int wpc = 1;
-        if (compact) {
-          static int per_bucket[4] = {0, 0, 0, 0}, parsed = 0;     // B200MJ_ACC_WARPS_B="4,3,2,2": warps per CTA by bucket (experiments)
-          if (!parsed) { parsed = 1; if (const char* e = getenv("B200MJ_ACC_WARPS_B")) sscanf(e, "%d%*c%d%*c%d%*c%d", &per_bucket[0], &per_bucket[1], &per_bucket[2], &per_bucket[3]); }
-          const int want = per_bucket[b] > 0 ? per_bucket[b] : (M->tn_nv ? acc_warps : 8);      // runtime-size kernels (__launch_bounds__(256)): whatever fills the SM
-          int cap = (int)((227 * 1024) / ws); if (cap > want) cap = want; if (M->tn_nv && cap > 4) cap = 4; if (cap < 1) cap = 1;
-          // as many resident warps per SM as 227 KB allow (CMU corridor, 37 KB per warp: two CTAs of 3 instead of one of 4); ties: the larger CTA
-          int best = 0;
-          for (int w = cap; w >= 1; w--) { const int res = (int)((227 * 1024) / ((w * ws) + 1024)) * w; if (res > best) { best = res; wpc = w; } }
-        }
-        const int grid = compact ? (cnt + wpc - 1) / wpc + (niter_split > 0 ? 1 : 0) : cnt;      // two classes: one more partial CTA
-        const int* bc = compact ? gcount + s * 8 + b : nullptr;
-        const int* bl = compact ? glist + (size_t)b * M->hand_batch : nullptr;
+        // warps per CTA: as many as fit 227 KB, at most acc_warps
+        const int want = M->tn_nv ? M->hooks.acc_warps : 8;      // runtime-size kernels (__launch_bounds__(256)): whatever fills the SM
+        int cap = (int)((227 * 1024) / ws); if (cap > want) cap = want; if (M->tn_nv && cap > 4) cap = 4; if (cap < 1) cap = 1;
+        // as many resident warps per SM as 227 KB allow (CMU corridor, 37 KB per warp: two CTAs of 3 instead of one of 4); ties: the larger CTA
+        int wpc = 1, best = 0;
+        for (int w = cap; w >= 1; w--) { const int res = (int)((227 * 1024) / ((w * ws) + 1024)) * w; if (res > best) { best = res; wpc = w; } }
+        const int grid = (cnt + wpc - 1) / wpc;
+        const int* bl = glist + (size_t)b * M->hand_batch;
         const Lay& la = last ? M->lay_accs_b[b] : M->lay_acc_b[b];
-        const int aflags = flags | ((compact && acc_sync && wpc > 1) ? (B200MJ_INTERNAL_ACC_SYNC | (acc_sync == 1 ? B200MJ_INTERNAL_ACC_SYNC_COARSE : 0)) : 0);
-        if (M->tn_nv) {
-          acc_kernel_fn fn = tn_kernel(M->tn_nv, last);
-          B200MJ_LAUNCH(fn, grid, 32 * wpc, ws * wpc + acc_pad, sb, M->dm, la, M->hand, M->hand2, *io, M->d_hand, M->d_hand2,
-                        e1, 0, s == 0, gt, le, aflags, e0, bc, bl, M->hand_batch, (compact && niter_split > 0) ? M->d_niter : nullptr);
-        } else if (last) B200MJ_LAUNCH(b200mj_acclast_kernel, grid, 32 * wpc, ws * wpc + acc_pad, sb, M->dm, la, M->hand, M->hand2, *io, M->d_hand, M->d_hand2,
-                                                                            e1, 0, s == 0, gt, le, aflags, e0, bc, bl, M->hand_batch, (compact && niter_split > 0) ? M->d_niter : nullptr);
-        else B200MJ_LAUNCH(b200mj_acc_kernel, grid, 32 * wpc, ws * wpc + acc_pad, sb, M->dm, la, M->hand, M->hand2, *io, M->d_hand, M->d_hand2,
-                                                                  e1, 0, s == 0, gt, le, aflags, e0, bc, bl, M->hand_batch, (compact && niter_split > 0) ? M->d_niter : nullptr);
+        acc_kernel_fn fn = M->tn_nv ? tn_kernel(M->tn_nv, last) : last ? (acc_kernel_fn)b200mj_acclast_kernel : (acc_kernel_fn)b200mj_acc_kernel;
+        B200MJ_LAUNCH(fn, grid, 32 * wpc, ws * wpc, sb, M->dm, la, M->hand, M->hand2, *io, M->d_hand, M->d_hand2, 0, s == 0, flags, gcount + b, bl);
         if (b > 0) cudaEventRecord(M->ev_acc[g][b], sb);
         g_launches++;
       }
       for (int b = 1; b < M->nbucket; b++) cudaStreamWaitEvent(sm, M->ev_acc[g][b], 0);   // join after the main-stream bucket is queued
     }
-    if (all_split) {
-      const Compact cp = compact_for(0);      // the next call's first acceleration launches read slot 0
-      B200MJ_LAUNCH((M->pos_big ? b200mj_posfinal_big_kernel : M->convex_pairs ? b200mj_posfinal_kernel : b200mj_posfinal_prim_kernel), gp, 32 * M->epb_pos, M->smem_pos * M->epb_pos + 64, sm, M->dm, M->lay_pos, M->hand, M->hand2, *io, M->d_hand, M->d_hand2,
-                                                                                    e1, 0, flags, want_sens && nstep == 1, e0, cp);
-      g_launches++;
-    }
+    const Compact cp = compact();      // the lists of the next call's first physics step
+    B200MJ_LAUNCH((M->pos_big ? b200mj_posfinal_big_kernel : M->convex_pairs ? b200mj_posfinal_kernel : b200mj_posfinal_prim_kernel), gp, 32 * M->epb_pos, M->smem_pos * M->epb_pos + 64, sm, M->dm, M->lay_pos, M->hand, M->hand2, *io, M->d_hand, M->d_hand2,
+                                                                                  e1, 0, flags, want_sens && nstep == 1, e0, cp);
+    g_launches++;
     if (g > 0) { cudaEventRecord(M->ev_join[g], sm); cudaStreamWaitEvent(st, M->ev_join[g], 0); }
   }
   if (cudaGetLastError() != cudaSuccess) return -5;
-  if (all_split) {
-    if (flags & B200MJ_STEP_FULL_FINAL) { M->reuse_ok = 1; M->reuse_qpos = io->qpos; M->reuse_batch = batch; M->reuse_flags = flags & ~B200MJ_STEP_REUSE_POS; M->reuse_has_dump = want_sens && nstep == 1; }
-    return 0;
-  }
-  return launch(M, io, batch, 1, flags, MODE_STEP, 0, stream);
+  if (flags & B200MJ_STEP_FULL_FINAL) { M->reuse_ok = 1; M->reuse_qpos = io->qpos; M->reuse_batch = batch; M->reuse_flags = flags & ~B200MJ_STEP_REUSE_POS; M->reuse_has_dump = want_sens && nstep == 1; }
+  return 0;
 }
 
 int b200mj_forward(const b200mj_model* M, const b200mj_io* io, int batch, int extra_disableflags, int flags, void* stream) {

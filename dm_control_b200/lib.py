@@ -7,7 +7,7 @@ import re
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_HERE)
-# B200MJ_SO: developer override (A/B runs of kernel variants built side by side, tools/ab_variants.sh); the default is the
+# B200MJ_SO: developer override (A/B runs of two builds of the library side by side); the default is the
 # in-tree library __graft_entry__.build() produces
 SO_PATH = os.environ.get('B200MJ_SO') or os.path.join(_HERE, 'csrc', 'libb200mj.so')
 HEADER = os.path.join(_ROOT, 'include', 'b200mj.h')

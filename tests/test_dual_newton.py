@@ -78,18 +78,10 @@ def test_dual_direction_matches_oracle_emulated():
   assert ref['pairs_ok'] and ref['worst'] < 1e-9, ref
 
 
-@pytest.mark.timeout(1800)
-def test_sparse_ldl_matches_oracle_emulated():
-  """B200MJ_SPARSE_LDL=1 (tree-sparse L'DL of M and M + h B, off by default: DESIGN.md 5) on the 62-dof CMU humanoid."""
-  out = _run('cmu_humanoid', 3, 6, 6, 1, B200MJ_SPARSE_LDL='1')
-  assert out['pairs_ok'] and out['worst'] < 1e-9, out
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize('name,B,ncontrol,nsub,env', [
     ('humanoid', 32, 30, 5, dict(B200MJ_TN='0', B200MJ_DUAL_MIN_NV='1')),      # dual form forced on (runtime-size kernels)
     ('cmu_humanoid', 16, 5, 6, dict()),                                          # default: dual form for nv = 62
-    ('cmu_humanoid', 8, 5, 6, dict(B200MJ_SPARSE_LDL='1')),                      # + tree-sparse L'DL (experimental, off by default)
 ])
 def test_dual_direction_matches_oracle_on_gpu(name, B, ncontrol, nsub, env):
   if os.environ.get('B200MJ_EMULATE_GPU') == '1':

@@ -87,24 +87,25 @@ def test_rollout(name, B, ncontrol, nsub, oracle_mod):
 
 
 def test_nstep_equals_repeated_steps_and_batch_independence(oracle_mod):
-  """engine_test.py:627-663 on the emulated kernels: step(3) is bitwise 3 x step(1); an environment's trajectory does
-  not depend on which batch it sits in."""
-  model = tm.load('humanoid')
-  q0, v0 = tm.initial_states(model, 'humanoid', 3, 5)
-  ctrl = np.random.RandomState(2).uniform(-1, 1, (3, model.nu))
-  def run(sel, chunks):
-    p = emu.EmuPhysics(model, len(sel))
-    p.data.qpos[:] = q0[sel]; p.data.qvel[:] = v0[sel]; p.forward(); p.data.ctrl[:] = ctrl[sel]
-    for n in chunks:
-      p.step(n)
-    return p.data.qpos.copy(), p.data.qvel.copy(), p.data.sensordata.copy()
-  a = run([0, 1, 2], [3])
-  b = run([0, 1, 2], [1, 1, 1])
-  c = run([1], [3])
-  for x, y in zip(a, b):
-    np.testing.assert_array_equal(x, y)
-  for x, y in zip(a, c):
-    np.testing.assert_array_equal(x[1:2], y)
+  """engine_test.py:627-663 on the emulated kernels: step(3) is bitwise 3 x step(1), and a call of more than 64
+  physics steps, step(70), bitwise 2 x step(35); an environment's trajectory does not depend on which batch it sits in."""
+  for name, whole, chunks in (('humanoid', [3], [1, 1, 1]), ('cheetah', [70], [35, 35])):
+    model = tm.load(name)
+    q0, v0 = tm.initial_states(model, name, 3, 5)
+    ctrl = np.random.RandomState(2).uniform(-1, 1, (3, model.nu))
+    def run(sel, chunks):
+      p = emu.EmuPhysics(model, len(sel))
+      p.data.qpos[:] = q0[sel]; p.data.qvel[:] = v0[sel]; p.forward(); p.data.ctrl[:] = ctrl[sel]
+      for n in chunks:
+        p.step(n)
+      return p.data.qpos.copy(), p.data.qvel.copy(), p.data.sensordata.copy()
+    a = run([0, 1, 2], whole)
+    b = run([0, 1, 2], chunks)
+    c = run([1], whole)
+    for x, y in zip(a, b):
+      np.testing.assert_array_equal(x, y)
+    for x, y in zip(a, c):
+      np.testing.assert_array_equal(x[1:2], y)
 
 
 def test_bad_control_and_divergence_warnings():
@@ -184,9 +185,9 @@ print(h.hexdigest())
 
 
 def test_launch_knobs_do_not_change_results():
-  """The fused kernel, the hybrid and the all-split path, any row-bucket partition, bucket launch order and
-  environment grouping are scheduling choices: every one of them must reproduce the default path bit for bit
-  (states, sensors, contacts, constraint forces, over rollouts with contacts)."""
+  """The fused and the split path, any row-bucket partition, the CTA widths of every kernel and the convex-pair
+  dispatch are scheduling choices: every one of them must reproduce the default path bit for bit (states, sensors,
+  contacts, constraint forces, over rollouts with contacts)."""
   import subprocess
   root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
   def digest(**env):
@@ -198,11 +199,9 @@ def test_launch_knobs_do_not_change_results():
   from concurrent.futures import ThreadPoolExecutor      # the variants are independent child processes: run them side by side
   pool = ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 2))
   ref_f = pool.submit(digest)
-  variants = (dict(B200MJ_BUCKETS='4,16'), dict(B200MJ_BUCKETS='6,12,24'), dict(B200MJ_BUCKET_ORDER='1'), dict(B200MJ_EPB_POS='2'),
-                # acceleration launches: one-warp CTAs, compacted lists with 2 / 4 warps, with / without phase barriers, two
-                # iteration-count classes per bucket: scheduling only
-                dict(B200MJ_COMPACT='0'), dict(B200MJ_ACC_WARPS='2'), dict(B200MJ_ACC_SYNC='0'), dict(B200MJ_ACC_SYNC='1'),
-                dict(B200MJ_NITER_SPLIT='3'), dict(B200MJ_NITER_SPLIT='2', B200MJ_ACC_WARPS='3'),
+  variants = (dict(B200MJ_BUCKETS='4,16'), dict(B200MJ_BUCKETS='6,12,24'), dict(B200MJ_EPB_POS='2'),
+                # acceleration launches: unsynchronised one-warp CTAs, phase-aligned CTAs of 2 warps (4: the default)
+                dict(B200MJ_ACC_WARPS='1'), dict(B200MJ_ACC_WARPS='2'),
                 # the emulator running the lanes of every block in descending instead of ascending order: a cross-lane
                 # dependency through shared memory that no collective or barrier separates would change the result
                 dict(B200MJ_EMU_ORDER='reverse'),
@@ -210,10 +209,10 @@ def test_launch_knobs_do_not_change_results():
                 dict(B200MJ_CVX_WARP='0'))
   futs = [(k, pool.submit(digest, **k)) for k in variants]
   # B200MJ_TN=0: the runtime-size acceleration kernels share their arithmetic with the fused kernel, so there the
-  # fused, hybrid and all-split paths must agree bit for bit as well
+  # fused and the split path must agree bit for bit as well
   ref0_f = pool.submit(digest, B200MJ_TN='0')
-  variants0 = (dict(B200MJ_SPLIT='0'), dict(B200MJ_SPLIT='1'), dict(B200MJ_BUCKETS='4,16'), dict(B200MJ_ENVS_PER_BLOCK='2', B200MJ_SPLIT='0'),
-               dict(B200MJ_SYNC_LEVEL='0', B200MJ_SPLIT='0'), dict(B200MJ_EMU_ORDER='reverse', B200MJ_SPLIT='0'))
+  variants0 = (dict(B200MJ_SPLIT='0'), dict(B200MJ_BUCKETS='4,16'), dict(B200MJ_ENVS_PER_BLOCK='2', B200MJ_SPLIT='0'),
+               dict(B200MJ_EMU_ORDER='reverse', B200MJ_SPLIT='0'))
   futs0 = [(k, pool.submit(digest, B200MJ_TN='0', **k)) for k in variants0]
   ref, ref0 = ref_f.result(), ref0_f.result()
   for knobs, f in futs:

@@ -50,16 +50,17 @@ def test_contact_force_equals_weight_on_gpu():
     assert abs(float(d.efc_force[0, a:a + 4].sum()) - float(forces[i, 0, 0])) < 1e-12
 
 
-@pytest.mark.parametrize('name', ['cheetah', 'cartpole', 'humanoid'])
-def test_nstep_equals_repeated_step_bitwise(name):
-  # dm_control/mujoco/engine_test.py:627-663 (Euler for cheetah/humanoid, RK4 for cartpole)
+@pytest.mark.parametrize('name,nstep', [('cheetah', 4), ('cartpole', 4), ('humanoid', 4), ('cheetah', 70)],
+                         ids=['cheetah', 'cartpole', 'humanoid', 'cheetah-70'])
+def test_nstep_equals_repeated_step_bitwise(name, nstep):
+  # dm_control/mujoco/engine_test.py:627-663 (Euler for cheetah/humanoid, RK4 for cartpole); 70: a call of more than 64 physics steps
   a, b = _phys(name, 8), _phys(name, 8)
   a.legacy_step = b.legacy_step = True
   for p in (a, b):
     _seed(p, name, 4)
     p.set_control(torch.full((p.model.nu,), 0.25, dtype=torch.float64))
-  a.step(4)
-  for _ in range(4):
+  a.step(nstep)
+  for _ in range(nstep):
     b.step()
   assert torch.equal(a.get_state(), b.get_state())
   assert torch.equal(a.data.qacc_warmstart, b.data.qacc_warmstart)
@@ -193,16 +194,16 @@ def test_fused_and_split_paths_agree_bitwise(monkeypatch):
   outs = []
   # B200MJ_TN=0: runtime-size acceleration kernels (they share their arithmetic with the fused kernel); the last run is the
   # default path, acceleration kernels with nv fixed at compile time (other summation order: equal to rounding noise only)
-  for split, tn in (('0', '0'), ('1', '0'), ('2', '0'), ('2', '1')):
+  for split, tn in (('0', '0'), ('1', '0'), ('1', '1')):
     env = dict(os.environ, B200MJ_SPLIT=split, B200MJ_TN=tn)
     r = subprocess.run([sys.executable, '-c', code], env=env, capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stderr[-2000:]
     outs.append(json.loads(r.stdout.strip().splitlines()[-1]))
-  assert outs[0] == outs[1] == outs[2]
+  assert outs[0] == outs[1]
   import numpy as np
-  assert outs[3]['n'] == outs[2]['n']
+  assert outs[2]['n'] == outs[1]['n']
   for f in ('q', 's'):
-    a, b = np.asarray(outs[3][f]), np.asarray(outs[2][f])
+    a, b = np.asarray(outs[2][f]), np.asarray(outs[1][f])
     assert np.abs(a - b).max() <= 1e-8 * (1 + np.abs(b).max()), (f, np.abs(a - b).max())
 
 

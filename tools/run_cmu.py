@@ -1,4 +1,4 @@
-"""A few control steps of the batched CMU corridor environment (profiling target: tools/profile_cmu.sh)."""
+"""A few control steps of the batched CMU corridor environment (a small target for timing and profiling runs)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
