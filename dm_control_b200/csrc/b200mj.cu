@@ -35,6 +35,8 @@
 
 #define FULL 0xffffffffu
 #define FOR_LANES(i, n) _Pragma("unroll 1") for (int i = lane; i < (n); i += 32)
+// dynamic shared memory one CTA may opt into on sm_90 (228 KB per SM, 1 KB of which is reserved per CTA)
+#define SMEM_MAX (227 * 1024)
 
 // ------------------------------------------------------------------------------------------------
 // device model view + workspace layout
@@ -87,8 +89,16 @@ struct Lay {
 // Per-environment row of the L2-resident handover buffer between the split position and acceleration kernels
 // (offsets in doubles).
 struct Hand { int M, J, efcD, aref, eqflag, bias, passive, tenlen, tenJ, counts, total; };
-// second row, written only in the last physics step: what the acceleration-stage sensors need from the position stage
-struct Hand2 { int xpos, xquat, xmat, xipos, scom, cinert, cdof, cdofdot, cvel, con, total; };
+// Second row, written only in the last physics step: what the acceleration-stage sensors need from the position stage.
+// X(field, doubles), with the model `m` and the contact count `ncon` in scope. The struct, its layout, the position
+// kernel's dump, the acceleration kernel's reload and the sensor-carrying acceleration workspace all expand this list.
+#define HAND2_FIELDS(X) X(xpos, 3 * m.nbody) X(xquat, 4 * m.nbody) X(xmat, 9 * m.nbody) X(xipos, 3 * m.nbody) \
+  X(scom, 3 * m.nbody) X(cinert, 10 * m.nbody) X(cdof, 6 * m.nv) X(cdofdot, 6 * m.nv) X(cvel, 6 * m.nbody) X(con, ncon * CON_STRIDE)
+#define HAND2_DECL(f, n) int f;
+struct Hand2 { HAND2_FIELDS(HAND2_DECL) int total; };
+#undef HAND2_DECL
+// the handover buffers of the split path and their row layouts: rows [hand_batch + SHADOW_ROWS][H.total], rows2 likewise
+struct Handover { Hand H; Hand2 H2; double* rows; double* rows2; };
 
 // Row-bucket compaction (split path): the position kernel appends every environment to the list of its row-count
 // bucket (count[b] = entries so far, list[b * cap ..]); the acceleration launch of a bucket then runs dense CTAs of
@@ -103,11 +113,9 @@ struct b200mj_model {
   // acceleration kernel: row-count buckets (workspace sized for rows_cap[b] constraint rows), plain and
   // sensor-carrying (last physics step of a fused step) variants
   int nbucket; int rows_cap[4]; Lay lay_acc_b[4], lay_accs_b[4]; size_t smem_acc_b[4], smem_accs_b[4];
-  Hand hand; Hand2 hand2;
-  double* d_hand2;
+  Handover ho; int hand_batch;
   // environment groups x row buckets run on their own streams (independent work: hides each launch's tail)
   cudaStream_t gmain[2], gaux[2][4]; cudaEvent_t ev_fork, ev_join[2], ev_pos[2], ev_acc[2][4]; int streams_ok;
-  double* d_hand; int hand_batch;
   int convex_pairs;                // some candidate pair needs cvx_capsule_box / cvx_pair (else: primitive-only position kernels)
   int* d_bcount; int* d_blist;     // compaction: counters [2 groups][4 buckets], lists [2 groups][4 buckets][hand_batch]
   // the trailing mj_step1 of the last split-path step left a complete handover for this (io, batch): see B200MJ_STEP_REUSE_POS
@@ -2573,6 +2581,23 @@ __device__ __forceinline__ void write_outputs(const Ctx& c, const b200mj_io& io,
 #undef OUT
 }
 
+// the state a physics step advances, workspace -> io (NVT: compile-time nv of the acceleration kernels, 0: runtime)
+template <int NVT>
+__device__ __forceinline__ void store_state(const Ctx& c, const b200mj_io& io, size_t e, double time) {
+  const DevModel& m = c.m; int lane = c.lane; const int nv = NVT > 0 ? NVT : m.nv;
+  FOR_LANES(i, m.nq) io.qpos[e * m.nq + i] = W(qpos)[i];
+  FOR_LANES(i, nv) { io.qvel[e * nv + i] = W(qvel)[i]; if (io.qacc_warmstart) io.qacc_warmstart[e * nv + i] = W(qaccws)[i]; }
+  FOR_LANES(i, m.na) io.act[e * m.na + i] = W(act)[i];
+  if (io.time && lane == 0) io.time[e] = time;
+}
+
+// adds a launch's warning counts (indexed by BMJ_WARN_*) to the environment's counters
+__device__ __forceinline__ void add_warnings(const b200mj_io& io, size_t e, int lane, const int (&n)[BMJ_NWARNING]) {
+  if (!io.warning || lane != 0) return;
+  int* w = io.warning + e * BMJ_NWARNING;
+  _Pragma("unroll") for (int k = 0; k < BMJ_NWARNING; k++) if (n[k]) w[k] += n[k];
+}
+
 enum { MODE_STEP = 0, MODE_FORWARD = 1 };
 
 // One launch = one warp per environment, `nstep` physics steps fused. Every stage function is inlined exactly
@@ -2581,8 +2606,9 @@ enum { MODE_STEP = 0, MODE_FORWARD = 1 };
 //   ordering one trailing [posvel] pass (= mj_step1 on the new state); MODE_FORWARD = one [posvel + acc] pass.
 // CVX: as for the position kernels (the primitive-only build shares narrowphase<false> with them, so the two paths stay bit-identical).
 template <bool CVX>
-__device__ __forceinline__ void step_kernel_body(const DevModel& m, const Lay& L, const b200mj_io& io,
-                   int batch, int nstep, int flags, int mode, int extra_disable, const uint8_t* env_mask) {
+__global__ void __launch_bounds__(256)
+step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ b200mj_io io,
+            int batch, int nstep, int flags, int mode, int extra_disable, const uint8_t* env_mask) {
   B200MJ_DYN_SMEM
   int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int env = blockIdx.x * (blockDim.x >> 5) + warp;
@@ -2600,7 +2626,7 @@ __device__ __forceinline__ void step_kernel_body(const DevModel& m, const Lay& L
   FOR_LANES(i, m.nu) W(ctrl)[i] = io.ctrl ? io.ctrl[e * m.nu + i] : 0.0;
   if (io.sensordata) FOR_LANES(i, m.nsensordata) W(sens)[i] = io.sensordata[e * m.nsensordata + i];
   double time = io.time ? io.time[e] : 0.0;
-  int w_contactfull = 0, w_cnstrfull = 0, w_badqpos = 0, w_badqvel = 0, w_badqacc = 0, w_badctrl = 0;
+  int warn[BMJ_NWARNING] = {};
   __syncwarp();
   const bool want_sens = (flags & B200MJ_STEP_SENSORS) != 0;
   const bool forward = mode == MODE_FORWARD;
@@ -2608,7 +2634,7 @@ __device__ __forceinline__ void step_kernel_body(const DevModel& m, const Lay& L
   const bool full_final = (flags & B200MJ_STEP_FULL_FINAL) != 0;
   const bool rk4 = m.integrator == BMJ_INT_RK4;
   // ---- control check (mj_step / mj_step2 / mj_forward all start from a finite ctrl) ----
-  if (check_bad(c, W(ctrl), m.nu)) { w_badctrl++; FOR_LANES(i, m.nu) W(ctrl)[i] = 0; __syncwarp(); }
+  if (check_bad(c, W(ctrl), m.nu)) { warn[BMJ_WARN_BADCTRL]++; FOR_LANES(i, m.nu) W(ctrl)[i] = 0; __syncwarp(); }
 
   int step_idx = 0, sub = 0;             // sub: Runge-Kutta stage 0..3 (always 0 for Euler)
   int r_ncon = 0, r_nefc = 0, r_niter = 0;   // reported statistics (first evaluation of a step)
@@ -2617,8 +2643,8 @@ __device__ __forceinline__ void step_kernel_body(const DevModel& m, const Lay& L
     if (final_pass && !legacy) break;
     const bool last = forward || step_idx == nstep - 1;
     if (!forward && sub == 0) {
-      if (check_bad(c, W(qpos), m.nq)) { w_badqpos++; reset_state(c, &time); }
-      if (check_bad(c, W(qvel), m.nv)) { w_badqvel++; reset_state(c, &time); }
+      if (check_bad(c, W(qpos), m.nq)) { warn[BMJ_WARN_BADQPOS]++; reset_state(c, &time); }
+      if (check_bad(c, W(qvel), m.nv)) { warn[BMJ_WARN_BADQVEL]++; reset_state(c, &time); }
     }
     // ---------------- position + velocity stage ----------------
     PHASE_SYNC();
@@ -2630,7 +2656,7 @@ __device__ __forceinline__ void step_kernel_body(const DevModel& m, const Lay& L
       int wfull = 0, cfull = 0;
       ncon = collision<CVX>(c, &wfull);
       nefc = make_constraint(c, ncon, &cfull);
-      w_contactfull += wfull; w_cnstrfull += cfull;
+      warn[BMJ_WARN_CONTACTFULL] += wfull; warn[BMJ_WARN_CNSTRFULL] += cfull;
     }
     fwd_velocity(c);
     const bool out_posvel = final_pass || forward || (!legacy && last && sub == 0);
@@ -2651,7 +2677,7 @@ __device__ __forceinline__ void step_kernel_body(const DevModel& m, const Lay& L
     if (live && (out_posvel || out_acc)) write_outputs(c, io, env, r_ncon, r_nefc, r_niter, out_posvel, out_acc, want_sens && out_posvel);
     if (final_pass || forward) break;
     // ---------------- integration ----------------
-    if (sub == 0 && check_bad(c, W(qacc), m.nv)) { w_badqacc++; reset_state(c, &time); step_idx++; continue; }
+    if (sub == 0 && check_bad(c, W(qacc), m.nv)) { warn[BMJ_WARN_BADQACC]++; reset_state(c, &time); step_idx++; continue; }
     if (!rk4) { euler_step<0>(c, &time); step_idx++; }
     else {
       // classic RK4 over (qpos, qvel, act): stage `sub` has just produced F_sub = (qvel, qacc, act_dot)
@@ -2684,34 +2710,13 @@ __device__ __forceinline__ void step_kernel_body(const DevModel& m, const Lay& L
     FOR_LANES(i, m.nq) io.qpos[e * m.nq + i] = W(qpos)[i];   // quaternions were normalised in place
   } else {
     if (!legacy && want_sens) { FOR_LANES(i, m.nsensordata) if (io.sensordata) io.sensordata[e * m.nsensordata + i] = W(sens)[i]; }
-    FOR_LANES(i, m.nq) io.qpos[e * m.nq + i] = W(qpos)[i];
-    FOR_LANES(i, m.nv) { io.qvel[e * m.nv + i] = W(qvel)[i]; if (io.qacc_warmstart) io.qacc_warmstart[e * m.nv + i] = W(qaccws)[i]; }
-    FOR_LANES(i, m.na) io.act[e * m.na + i] = W(act)[i];
-    if (io.time && lane == 0) io.time[e] = time;
+    store_state<0>(c, io, e, time);
   }
-  if (io.warning && lane == 0) {
-    int* w = io.warning + e * BMJ_NWARNING;
-    if (w_contactfull) w[BMJ_WARN_CONTACTFULL] += w_contactfull;
-    if (w_cnstrfull) w[BMJ_WARN_CNSTRFULL] += w_cnstrfull;
-    if (w_badqpos) w[BMJ_WARN_BADQPOS] += w_badqpos;
-    if (w_badqvel) w[BMJ_WARN_BADQVEL] += w_badqvel;
-    if (w_badqacc) w[BMJ_WARN_BADQACC] += w_badqacc;
-    if (w_badctrl) w[BMJ_WARN_BADCTRL] += w_badctrl;
-  }
-}
-extern "C" __global__ void __launch_bounds__(256)
-b200mj_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ b200mj_io io,
-                   int batch, int nstep, int flags, int mode, int extra_disable, const uint8_t* env_mask) {
-  step_kernel_body<true>(m, L, io, batch, nstep, flags, mode, extra_disable, env_mask);
-}
-extern "C" __global__ void __launch_bounds__(256)
-b200mj_step_prim_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ b200mj_io io,
-                        int batch, int nstep, int flags, int mode, int extra_disable, const uint8_t* env_mask) {
-  step_kernel_body<false>(m, L, io, batch, nstep, flags, mode, extra_disable, env_mask);
+  add_warnings(io, e, lane, warn);
 }
 
 // ------------------------------------------------------------------------------------------------
-// Split path: the same stage functions in two smaller kernels. A pass is  [b200mj_pos_kernel -> b200mj_acc_kernel];
+// Split path: the same stage functions in two smaller kernels. A pass is  [pos_kernel -> acc_kernel];
 // M, efc_J, efc_D, aref, bias, passive (and the tendon tables) travel through an L2-resident handover row, the
 // state through the io arrays. Smaller code footprint and workspace per kernel => 2x the resident warps.
 // Used for the first nstep-1 physics steps of a fused step() when no applied forces are routed in; the last step
@@ -2719,10 +2724,20 @@ b200mj_step_prim_kernel(const __grid_constant__ DevModel m, const __grid_constan
 // ------------------------------------------------------------------------------------------------
 // FINAL = the trailing mj_step1 of the legacy ordering (subtree velocities, position/velocity sensors, outputs);
 // otherwise the position/velocity half of a physics step, optionally dumping what the acceleration-stage sensors need.
-template <bool FINAL, bool CVX>
-__device__ __forceinline__ void pos_kernel_body(const DevModel& m, const Lay& L, const Hand& H, const Hand2& H2, const b200mj_io& io,
-                                                double* hand, double* hand2, int batch, int extra_disable, int flags, int dump, int env0,
-                                                const Compact& cp) {
+// BUILD picks the narrow phase and the launch bounds:
+//   POS_CVX (160, 2): at most five phase-aligned warps per CTA and a 204-register budget, so that two CTAs share an SM
+//     (shared memory allows no more); the rarely taken convex narrow phase (cvx_mpr) would otherwise set the kernel's
+//     register count to 255 and halve occupancy
+//   POS_PRIM (160, 3): models whose candidate pairs are all analytic primitive pairs (no convex code, no stack spills):
+//     three CTAs per SM
+//   POS_BIG (224, 1): large models (CMU corridor: 30 KB of position workspace per environment, one CTA per SM either
+//     way): up to seven phase-aligned warps in that one CTA and the full register budget
+enum { POS_PRIM, POS_CVX, POS_BIG };
+template <bool FINAL, int BUILD>
+__global__ void __launch_bounds__(BUILD == POS_BIG ? 224 : 160, BUILD == POS_PRIM ? 3 : BUILD == POS_CVX ? 2 : 1)
+pos_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Handover ho,
+           const __grid_constant__ b200mj_io io, int batch, int flags, int dump, int env0, const __grid_constant__ Compact cp) {
+  constexpr bool CVX = BUILD != POS_PRIM;
   B200MJ_DYN_SMEM
   int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int env = env0 + blockIdx.x * (blockDim.x >> 5) + warp;      // this launch covers environments [env0, batch)
@@ -2732,13 +2747,14 @@ __device__ __forceinline__ void pos_kernel_body(const DevModel& m, const Lay& L,
   // rewrite identical values and skip the warning counters.
   const bool live = env < batch;
   if (!live) env = batch - 1;
-  Ctx c(m, L, smem + (size_t)warp * L.total, lane, m.disableflags | extra_disable, 0);
+  Ctx c(m, L, smem + (size_t)warp * L.total, lane, m.disableflags, 0);
   c.set_env(env, io);
   size_t e = (size_t)env;
   // A shadow warp gets a handover row of its own: the stages read back what they wrote there (raw-contact staging, Jacobian rows), so
   // sharing the live environment's row would race; the io arrays are only ever overwritten with identical values.
   const size_t hr = live ? e : (size_t)(cp.shadow_row + warp);
-  double* hrow = hand + hr * H.total;
+  const Hand& H = ho.H;
+  double* hrow = ho.rows + hr * H.total;
   c.pM = hrow + H.M; c.pJ = hrow + H.J; c.pD = hrow + H.efcD; c.pAref = hrow + H.aref; c.pBias = hrow + H.bias;
   c.pPassive = hrow + H.passive; c.pEq = reinterpret_cast<int*>(hrow + H.eqflag);
   c.stage = hrow + H.J;         // raw-contact staging: the row's Jacobian block (L2), written only later by make_constraint
@@ -2746,10 +2762,10 @@ __device__ __forceinline__ void pos_kernel_body(const DevModel& m, const Lay& L,
   FOR_LANES(i, m.nv) W(qvel)[i] = io.qvel[e * m.nv + i];
   const bool want_sens = FINAL && (flags & B200MJ_STEP_SENSORS) != 0;
   __syncwarp();
-  int w_badqpos = 0, w_badqvel = 0, did_reset = 0;
-  if (check_bad(c, W(qpos), m.nq)) { w_badqpos++; did_reset = 1; }
-  if (check_bad(c, W(qvel), m.nv)) { w_badqvel++; did_reset = 1; }
-  if (did_reset) {
+  int warn[BMJ_NWARNING] = {};
+  warn[BMJ_WARN_BADQPOS] = check_bad(c, W(qpos), m.nq);
+  warn[BMJ_WARN_BADQVEL] = check_bad(c, W(qvel), m.nv);
+  if (warn[BMJ_WARN_BADQPOS] || warn[BMJ_WARN_BADQVEL]) {
     FOR_LANES(i, m.nq) W(qpos)[i] = m.qpos0[i];
     FOR_LANES(i, m.nv) { W(qvel)[i] = 0; io.qvel[e * m.nv + i] = 0; if (io.qacc_warmstart) io.qacc_warmstart[e * m.nv + i] = 0; }
     FOR_LANES(i, m.na) io.act[e * m.na + i] = 0;
@@ -2784,11 +2800,9 @@ __device__ __forceinline__ void pos_kernel_body(const DevModel& m, const Lay& L,
     copy_row(hrow + H.tenJ, W(tenJ), m.ntendon * m.ldv, lane);
     if (lane == 0) { int* cnt = reinterpret_cast<int*>(hrow + H.counts); cnt[0] = ncon; cnt[1] = nefc; }
     if (dump) {
-      double* d2 = hand2 + hr * H2.total;
-#define DUMP(dst, src, n) copy_row(d2 + H2.dst, W(src), (n), lane);
-      DUMP(xpos, xpos, 3 * m.nbody) DUMP(xquat, xquat, 4 * m.nbody) DUMP(xmat, xmat, 9 * m.nbody) DUMP(xipos, xipos, 3 * m.nbody)
-      DUMP(scom, scom, 3 * m.nbody) DUMP(cinert, cinert, 10 * m.nbody) DUMP(cdof, cdof, 6 * m.nv) DUMP(cdofdot, cdofdot, 6 * m.nv)
-      DUMP(cvel, cvel, 6 * m.nbody) DUMP(con, con, ncon * CON_STRIDE)
+      double* d2 = ho.rows2 + hr * ho.H2.total;
+#define DUMP(f, n) copy_row(d2 + ho.H2.f, W(f), (n), lane);
+      HAND2_FIELDS(DUMP)
 #undef DUMP
     }
   }
@@ -2809,65 +2823,22 @@ __device__ __forceinline__ void pos_kernel_body(const DevModel& m, const Lay& L,
     __syncthreads();
     if (live && lane == 0) cp.list[(size_t)b * cp.cap + cta[4 + b] + my] = env;
   }
-  if (live && io.warning && lane == 0) {
-    int* w = io.warning + e * BMJ_NWARNING;
-    if (wfull) w[BMJ_WARN_CONTACTFULL] += 1;
-    if (cfull) w[BMJ_WARN_CNSTRFULL] += 1;
-    if (w_badqpos) w[BMJ_WARN_BADQPOS] += 1;
-    if (w_badqvel) w[BMJ_WARN_BADQVEL] += 1;
+  if (live) {
+    warn[BMJ_WARN_CONTACTFULL] = wfull; warn[BMJ_WARN_CNSTRFULL] = cfull;
+    add_warnings(io, e, lane, warn);
   }
 }
 
-// (160, 2): at most five phase-aligned warps per CTA and a 204-register budget, so that two CTAs share an SM (shared memory
-// allows no more); the
-// rarely taken convex narrow phase (cvx_mpr) would otherwise set the kernel's register count to 255 and halve occupancy
-extern "C" __global__ void __launch_bounds__(160, 2)
-b200mj_pos_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Hand H,
-                  const __grid_constant__ Hand2 H2, const __grid_constant__ b200mj_io io, double* hand, double* hand2, int batch,
-                  int extra_disable, int flags, int dump, int env0, const __grid_constant__ Compact cp) {
-  pos_kernel_body<false, true>(m, L, H, H2, io, hand, hand2, batch, extra_disable, flags, dump, env0, cp);
-}
-extern "C" __global__ void __launch_bounds__(160, 2)
-b200mj_posfinal_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Hand H,
-                       const __grid_constant__ Hand2 H2, const __grid_constant__ b200mj_io io, double* hand, double* hand2, int batch,
-                       int extra_disable, int flags, int dump, int env0, const __grid_constant__ Compact cp) {
-  pos_kernel_body<true, true>(m, L, H, H2, io, hand, hand2, batch, extra_disable, flags, dump, env0, cp);
-}
-
-// large models (CMU corridor: 30 KB of position workspace per environment, one CTA per SM either way): up to seven
-// phase-aligned warps in that one CTA and the full register budget
-extern "C" __global__ void __launch_bounds__(224, 1)
-b200mj_pos_big_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Hand H,
-                      const __grid_constant__ Hand2 H2, const __grid_constant__ b200mj_io io, double* hand, double* hand2, int batch,
-                      int extra_disable, int flags, int dump, int env0, const __grid_constant__ Compact cp) {
-  pos_kernel_body<false, true>(m, L, H, H2, io, hand, hand2, batch, extra_disable, flags, dump, env0, cp);
-}
-extern "C" __global__ void __launch_bounds__(224, 1)
-b200mj_posfinal_big_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Hand H,
-                           const __grid_constant__ Hand2 H2, const __grid_constant__ b200mj_io io, double* hand, double* hand2, int batch,
-                           int extra_disable, int flags, int dump, int env0, const __grid_constant__ Compact cp) {
-  pos_kernel_body<true, true>(m, L, H, H2, io, hand, hand2, batch, extra_disable, flags, dump, env0, cp);
-}
-
-// the same for models whose candidate pairs are all analytic primitive pairs (121 registers, no stack spills): three CTAs per SM
-extern "C" __global__ void __launch_bounds__(160, 3)
-b200mj_pos_prim_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Hand H,
-                  const __grid_constant__ Hand2 H2, const __grid_constant__ b200mj_io io, double* hand, double* hand2, int batch,
-                  int extra_disable, int flags, int dump, int env0, const __grid_constant__ Compact cp) {
-  pos_kernel_body<false, false>(m, L, H, H2, io, hand, hand2, batch, extra_disable, flags, dump, env0, cp);
-}
-extern "C" __global__ void __launch_bounds__(160, 3)
-b200mj_posfinal_prim_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Hand H,
-                       const __grid_constant__ Hand2 H2, const __grid_constant__ b200mj_io io, double* hand, double* hand2, int batch,
-                       int extra_disable, int flags, int dump, int env0, const __grid_constant__ Compact cp) {
-  pos_kernel_body<true, false>(m, L, H, H2, io, hand, hand2, batch, extra_disable, flags, dump, env0, cp);
-}
-
-// LAST = last physics step of a fused step(): acceleration-stage sensors and outputs are produced here
+// LAST = last physics step of a fused step(): acceleration-stage sensors and outputs are produced here.
+// NVT = 0: nv at run time (any model; CTAs of up to 8 warps). Otherwise nv fixed at compile time (register-resident
+// algebra, tn_* above), one instantiation per nv of B200MJ_NV_LIST — the dofs of the benchmark configurations (cheetah 9,
+// quadruped 22, humanoid 27) and a few common small sizes — built for at most 4 warps per CTA. Same arguments, same
+// handover format.
+#define B200MJ_NV_LIST(X) X(6) X(9) X(12) X(18) X(22) X(27)
 template <bool LAST, int NVT>
-__device__ __forceinline__ void acc_kernel_body(const DevModel& m, const Lay& L, const Hand& H, const Hand2& H2, const b200mj_io& io,
-                                                const double* hand, const double* hand2, int extra_disable, int first_pass, int flags,
-                                                const int* bucket_count, const int* bucket_list) {
+__global__ void __launch_bounds__(NVT > 0 ? 128 : 256, NVT > 0 ? 4 : 0)
+acc_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Handover ho,
+           const __grid_constant__ b200mj_io io, int first_pass, int flags, const int* bucket_count, const int* bucket_list) {
   B200MJ_DYN_SMEM
   int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // One launch per row-count bucket: the CTAs walk the bucket's environment list (*bucket_count entries), which the
@@ -2884,10 +2855,11 @@ __device__ __forceinline__ void acc_kernel_body(const DevModel& m, const Lay& L,
   }
   const int env = bucket_list[k];
   size_t e = (size_t)env;
-  const double* hrow = hand + e * H.total;
+  const Hand& H = ho.H;
+  const double* hrow = ho.rows + e * H.total;
   const int* cnt = reinterpret_cast<const int*>(hrow + H.counts);
   const int ncon = cnt[0], nefc = cnt[1];
-  Ctx c(m, L, smem + (size_t)warp * L.total, lane, m.disableflags | extra_disable, sync);
+  Ctx c(m, L, smem + (size_t)warp * L.total, lane, m.disableflags, sync);
   c.set_env(env, io);
   const int nv = NVT > 0 ? NVT : m.nv, ld = NVT > 0 ? (NVT | 1) : m.ldv;
   // ---- load state + handover ----
@@ -2907,8 +2879,8 @@ __device__ __forceinline__ void acc_kernel_body(const DevModel& m, const Lay& L,
   const bool want_sens = LAST && (flags & B200MJ_STEP_SENSORS) != 0;
   double time = io.time ? io.time[e] : 0.0;
   __syncwarp();
-  int w_badctrl = 0, w_badqacc = 0;
-  if (check_bad(c, W(ctrl), m.nu)) { w_badctrl = first_pass; FOR_LANES(i, m.nu) W(ctrl)[i] = 0; __syncwarp(); }
+  int warn[BMJ_NWARNING] = {};
+  if (check_bad(c, W(ctrl), m.nu)) { warn[BMJ_WARN_BADCTRL] = first_pass; FOR_LANES(i, m.nu) W(ctrl)[i] = 0; __syncwarp(); }
   fwd_actuation(c);
   b200mj_io io_noforce = io; io_noforce.qfrc_applied = nullptr; io_noforce.xfrc_applied = nullptr;
   if (sync) __syncthreads();
@@ -2918,30 +2890,20 @@ __device__ __forceinline__ void acc_kernel_body(const DevModel& m, const Lay& L,
   if (LAST && live) write_outputs(c, io, env, ncon, nefc, niter, false, true, false);
   if (want_sens) FOR_LANES(i, nv) W(vold)[i] = W(qvel)[i];
   if (sync) __syncthreads();
-  if (check_bad(c, W(qacc), nv)) { w_badqacc = 1; reset_state(c, &time); }
+  if (check_bad(c, W(qacc), nv)) { warn[BMJ_WARN_BADQACC] = 1; reset_state(c, &time); }
   else euler_step<NVT>(c, &time);
   if (!live) return;      // shadows: no stores (the sensor epilogue below has no barriers)
-  // ---- store state ----
-  FOR_LANES(i, m.nq) io.qpos[e * m.nq + i] = W(qpos)[i];
-  FOR_LANES(i, nv) { io.qvel[e * nv + i] = W(qvel)[i]; if (io.qacc_warmstart) io.qacc_warmstart[e * nv + i] = W(qaccws)[i]; }
-  FOR_LANES(i, m.na) io.act[e * m.na + i] = W(act)[i];
-  if (io.time && lane == 0) io.time[e] = time;
-  if (io.warning && lane == 0) {
-    int* w = io.warning + e * BMJ_NWARNING;
-    if (w_badctrl) w[BMJ_WARN_BADCTRL] += 1;
-    if (w_badqacc) w[BMJ_WARN_BADQACC] += 1;
-  }
+  store_state<NVT>(c, io, e, time);
+  add_warnings(io, e, lane, warn);
   if (want_sens) {
     // Acceleration-stage sensors of the step just taken (MuJoCo evaluates them in mj_forward, before the state
     // advances): the solver's storage is dead now, so the position-stage dump is loaded over it (a workspace that
     // held both at once allowed 6 instead of 14 environments per SM).
     __syncwarp();
     FOR_LANES(i, nv) W(qvel)[i] = W(vold)[i];
-    const double* d2 = hand2 + e * H2.total;
-#define UNDUMP(dst, src, n) copy_row(W(dst), d2 + H2.src, (n), lane);
-    UNDUMP(xpos, xpos, 3 * m.nbody) UNDUMP(xquat, xquat, 4 * m.nbody) UNDUMP(xmat, xmat, 9 * m.nbody) UNDUMP(xipos, xipos, 3 * m.nbody)
-    UNDUMP(scom, scom, 3 * m.nbody) UNDUMP(cinert, cinert, 10 * m.nbody) UNDUMP(cdof, cdof, 6 * m.nv) UNDUMP(cdofdot, cdofdot, 6 * m.nv)
-    UNDUMP(cvel, cvel, 6 * m.nbody) UNDUMP(con, con, ncon * CON_STRIDE)
+    const double* d2 = ho.rows2 + e * ho.H2.total;
+#define UNDUMP(f, n) copy_row(W(f), d2 + ho.H2.f, (n), lane);
+    HAND2_FIELDS(UNDUMP)
 #undef UNDUMP
     if (io.sensordata) FOR_LANES(i, m.nsensordata) W(sens)[i] = io.sensordata[e * m.nsensordata + i];
     __syncwarp();
@@ -2951,46 +2913,41 @@ __device__ __forceinline__ void acc_kernel_body(const DevModel& m, const Lay& L,
   }
 }
 
-extern "C" __global__ void __launch_bounds__(256)
-b200mj_acc_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Hand H,
-                  const __grid_constant__ Hand2 H2, const __grid_constant__ b200mj_io io, const double* hand, const double* hand2,
-                  int extra_disable, int first_pass, int flags, const int* bucket_count, const int* bucket_list) {
-  acc_kernel_body<false, 0>(m, L, H, H2, io, hand, hand2, extra_disable, first_pass, flags, bucket_count, bucket_list);
-}
-extern "C" __global__ void __launch_bounds__(256)
-b200mj_acclast_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Hand H,
-                      const __grid_constant__ Hand2 H2, const __grid_constant__ b200mj_io io, const double* hand, const double* hand2,
-                  int extra_disable, int first_pass, int flags, const int* bucket_count, const int* bucket_list) {
-  acc_kernel_body<true, 0>(m, L, H, H2, io, hand, hand2, extra_disable, first_pass, flags, bucket_count, bucket_list);
-}
-
-// Acceleration kernels with nv fixed at compile time (register-resident algebra, tn_* above). One instantiation per
-// nv of B200MJ_NV_LIST — the dofs of the benchmark configurations (cheetah 9, quadruped 22, humanoid 27) and a few
-// common small sizes; any other model runs the runtime-size kernels above. Same arguments, same handover format.
-#define B200MJ_NV_LIST(X) X(6) X(9) X(12) X(18) X(22) X(27)
-template <bool LAST, int NVT>
-__global__ void __launch_bounds__(128, 4)
-b200mj_acc_tn_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Hand H,
-                     const __grid_constant__ Hand2 H2, const __grid_constant__ b200mj_io io, const double* hand, const double* hand2,
-                     int extra_disable, int first_pass, int flags, const int* bucket_count, const int* bucket_list) {
-  acc_kernel_body<LAST, NVT>(m, L, H, H2, io, hand, hand2, extra_disable, first_pass, flags, bucket_count, bucket_list);
-}
-
 // ------------------------------------------------------------------------------------------------
 // host side of the C ABI
 // ------------------------------------------------------------------------------------------------
 static int64_t g_launches = 0;
 
-typedef void (*acc_kernel_fn)(const DevModel, const Lay, const Hand, const Hand2, const b200mj_io, const double*, const double*,
-                              int, int, int, const int*, const int*);
-// the compile-time-size acceleration kernel for nv dofs, or nullptr
-static acc_kernel_fn tn_kernel(int nv, bool last) {
-  switch (nv) {
-#define TN_CASE(n) case n: return last ? (acc_kernel_fn)b200mj_acc_tn_kernel<true, n> : (acc_kernel_fn)b200mj_acc_tn_kernel<false, n>;
-    B200MJ_NV_LIST(TN_CASE)
-#undef TN_CASE
+typedef decltype(&step_kernel<true>) step_kernel_fn;
+typedef decltype(&pos_kernel<false, POS_CVX>) pos_kernel_fn;
+typedef decltype(&acc_kernel<false, 0>) acc_kernel_fn;
+
+static step_kernel_fn step_kernel_for(const b200mj_model* M) { return M->convex_pairs ? step_kernel<true> : step_kernel<false>; }
+
+// final: the trailing mj_step1
+static pos_kernel_fn pos_kernel_for(const b200mj_model* M, bool final) {
+  if (M->pos_big) return final ? pos_kernel<true, POS_BIG> : pos_kernel<false, POS_BIG>;
+  if (M->convex_pairs) return final ? pos_kernel<true, POS_CVX> : pos_kernel<false, POS_CVX>;
+  return final ? pos_kernel<true, POS_PRIM> : pos_kernel<false, POS_PRIM>;
+}
+
+// the acceleration kernel for a compile-time size of nvt dofs (0: the runtime-size kernel), or nullptr where
+// B200MJ_NV_LIST has no kernel for nvt
+static acc_kernel_fn acc_kernel_for(int nvt, bool last) {
+  switch (nvt) {
+#define NV_CASE(n) case n: return last ? acc_kernel<true, n> : acc_kernel<false, n>;
+    NV_CASE(0) B200MJ_NV_LIST(NV_CASE)
+#undef NV_CASE
     default: return nullptr;
   }
+}
+
+// Lets every kernel the model's current layout can launch use up to SMEM_MAX of dynamic shared memory. Runs again
+// whenever the layout is rebuilt: a change of capacities can move the model to another position-kernel build.
+static void allow_shared_memory(const b200mj_model* M) {
+  const void* kernels[] = {(const void*)step_kernel_for(M), (const void*)pos_kernel_for(M, false), (const void*)pos_kernel_for(M, true),
+                           (const void*)acc_kernel_for(M->tn_nv, false), (const void*)acc_kernel_for(M->tn_nv, true)};
+  for (const void* k : kernels) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
 }
 
 // Environment overrides, read once per model. Each is a test hook that steers a model onto a path it would not take by
@@ -3031,6 +2988,8 @@ static void build_layout(b200mj_model* M) {
   auto take = [&](int n) { int r = o; o += (n + 1) & ~1; return r; };   // keep 16-byte alignment
   int nv = m.nv, nb = m.nbody, ld = m.ldv, nj = m.njmax;
   const int ntri = nv * (nv + 1) / 2;   // packed lower triangle (M, H)
+  // efc_J; with candidate pairs at least STAGE_DOUBLES, where the narrow phase stages its raw contacts
+  const int jcap = (m.npair > 0 && nj * ld < STAGE_DOUBLES) ? STAGE_DOUBLES : nj * ld;
   L.qpos = take(m.nq); L.qvel = take(nv); L.act = take(m.na); L.ctrl = take(m.nu); L.qaccws = take(nv); L.actdot = take(m.na);
   L.xpos = take(3 * nb); L.xquat = take(4 * nb); L.xmat = take(9 * nb); L.xipos = take(3 * nb);
   L.scom = take(3 * nb); L.slinvel = take(3 * nb);
@@ -3045,7 +3004,7 @@ static void build_layout(b200mj_model* M) {
   L.H = h0;
   L.tenlen = take(m.ntendon); L.tenJ = take(m.ntendon * ld); L.actforce = take(m.nu);
   L.M = take(ntri); L.dinv = take(nv);
-  L.J = take((m.npair > 0 && nj * ld < STAGE_DOUBLES) ? STAGE_DOUBLES : nj * ld); L.efcD = take(nj); L.efcSD = take(nj); L.aref = take(nj); L.jar = take(nj); L.jv = take(nj);
+  L.J = take(jcap); L.efcD = take(nj); L.efcSD = take(nj); L.aref = take(nj); L.jar = take(nj); L.jv = take(nj);
   L.force = take(nj); L.eqflag = take((nj + 1) / 2); L.actlist = take((nj + 1) / 2);
   L.bias = take(nv); L.passive = take(nv); L.qfact = take(nv); L.smooth = take(nv); L.qaccs = take(nv); L.qacc = take(nv);
   L.qcon = take(nv); L.Ma = take(nv); L.grad = take(nv); L.search = take(nv); L.Mv = take(nv); L.tmpv = take(nv);
@@ -3060,7 +3019,7 @@ static void build_layout(b200mj_model* M) {
   M->smem_per_env = (size_t)o * sizeof(double);
   // One CTA per SM holding as many environments (= warps) as the 227 KB of shared memory allow, at most 8: the
   // warps of a CTA are phase-aligned with barriers and so share their instruction fetches.
-  int best = (int)((227 * 1024) / (M->smem_per_env ? M->smem_per_env : 1));
+  int best = (int)(SMEM_MAX / (M->smem_per_env ? M->smem_per_env : 1));
   if (best > 8) best = 8;
   if (M->hooks.envs_per_block >= 1 && M->hooks.envs_per_block <= best) best = M->hooks.envs_per_block;
   M->envs_per_block = best;
@@ -3069,7 +3028,7 @@ static void build_layout(b200mj_model* M) {
   {
     Lay& P = M->lay_pos; memset(&P, 0, sizeof(P));
     o = 0;
-    // Lifetimes (pos_kernel_body): kinematics -> collision -> com_pos -> crb_and_factor -> make_constraint -> fwd_velocity [-> subtree_vel,
+    // Lifetimes (pos_kernel): kinematics -> collision -> com_pos -> crb_and_factor -> make_constraint -> fwd_velocity [-> subtree_vel,
     // sensors]. Storage shared along that line, so that three 5-warp CTAs fit one SM (humanoid: 14.3 KB per environment, was 19.2):
     //   [gxpos gxmat]      dead after collision  ==  crb (crb_and_factor), then cacc, cfrc (fwd_velocity), then slinvel, sens (trailing step1)
     //   [xanchor xaxis]    dead after com_pos    ==  cdofdot (fwd_velocity)
@@ -3106,6 +3065,7 @@ static void build_layout(b200mj_model* M) {
     // dual form of the Newton direction in the runtime-size kernels from dual_min_nv dofs on (32: the two-rows-per-lane
     // factorisation)
     const int dual_min_nv = M->hooks.dual_min_nv;
+    const int ncon = m.nconmax;      // HAND2_FIELDS: room for every contact
     auto tri_host = [](int i) { return (i * (i + 1)) / 2; };
     auto acc_layout = [&](Lay& A, int rows, bool with_sens) {
       memset(&A, 0, sizeof(A));
@@ -3119,24 +3079,24 @@ static void build_layout(b200mj_model* M) {
       A.mglobal = (!M->tn_nv && nv >= 32) ? 1 : 0;
       A.M = take(A.mglobal ? 0 : ntri); A.H = take(ntri); A.dinv = take(nv);
       // dual form with few rows: J's workspace copy aliases H (dual_prepare), so that seven CMU environments fit an SM
-      const bool will_dual = dual_min_nv > 0 && !M->tn_nv && nv >= dual_min_nv && rows <= 32 && m.solver == BMJ_SOL_NEWTON;
-      const int dneed = rows * rows + tri_host(rows) + 3 * rows + 2;
-      A.jalias = (will_dual && rows * ld + dneed <= ntri) ? 1 : 0;
+      const bool dual = dual_min_nv > 0 && !M->tn_nv && nv >= dual_min_nv && rows <= 32 && m.solver == BMJ_SOL_NEWTON;
+      const int dneed = rows * rows + tri_host(rows) + 3 * rows + 2;      // dS
+      A.jalias = (dual && rows * ld + dneed <= ntri) ? 1 : 0;
       A.J = A.jalias ? A.H : take(rows * ld); A.efcD = take(rows); A.efcSD = take(rows); A.aref = take(rows); A.jar = take(rows); A.jv = take(rows);
       A.eqflag = take((rows + 1) / 2); A.actlist = take((rows + 1) / 2);
       A.bias = take(nv); A.passive = take(nv); A.qfact = take(nv); A.smooth = take(nv); A.qaccs = take(nv);
       A.qcon = take(nv); A.Ma = take(nv); A.grad = take(nv); A.search = take(nv); A.Mv = take(nv); A.tmpv = take(nv);
-      if (dual_min_nv > 0 && !M->tn_nv && nv >= dual_min_nv && rows <= 32 && m.solver == BMJ_SOL_NEWTON) {
+      if (dual) {
         A.dual = 1; A.drows = rows; A.dV = take(rows * ld);
-        const int need = rows * rows + tri_host(rows) + 3 * rows + 2;
-        A.dS = A.jalias ? A.H + ((rows * ld + 1) & ~1) : (need <= ntri ? A.H : take(need));
+        A.dS = A.jalias ? A.H + ((rows * ld + 1) & ~1) : (dneed <= ntri ? A.H : take(dneed));
       }
       if (with_sens) {
         const int acc_end = o;
         o = u0;
-        A.xpos = take(3 * nb); A.xquat = take(4 * nb); A.xmat = take(9 * nb); A.xipos = take(3 * nb); A.scom = take(3 * nb);
-        A.cinert = take(10 * nb); A.cdof = take(6 * nv); A.cdofdot = take(6 * nv); A.cvel = take(6 * nb);
-        A.cacc = take(6 * nb); A.cfrc = take(6 * nb); A.cfrcext = take(6 * nb); A.con = take(m.nconmax * CON_STRIDE);
+#define TAKE_DUMP(f, n) A.f = take(n);
+        HAND2_FIELDS(TAKE_DUMP)
+#undef TAKE_DUMP
+        A.cacc = take(6 * nb); A.cfrc = take(6 * nb); A.cfrcext = take(6 * nb);
         A.sens = take(m.nsensordata);
         if (o < acc_end) o = acc_end;
       }
@@ -3166,28 +3126,41 @@ static void build_layout(b200mj_model* M) {
       M->smem_accs_b[bi] = acc_layout(M->lay_accs_b[bi], cap, true);
       if (cap == nj) break;
     }
-    Hand& Hd = M->hand;
+    Hand& Hd = M->ho.H;
     o = 0;
-    Hd.M = take(ntri); Hd.J = take((m.npair > 0 && nj * ld < STAGE_DOUBLES) ? STAGE_DOUBLES : nj * ld); Hd.efcD = take(nj); Hd.aref = take(nj); Hd.eqflag = take((nj + 1) / 2);
+    Hd.M = take(ntri); Hd.J = take(jcap); Hd.efcD = take(nj); Hd.aref = take(nj); Hd.eqflag = take((nj + 1) / 2);
     Hd.bias = take(nv); Hd.passive = take(nv); Hd.tenlen = take(m.ntendon); Hd.tenJ = take(m.ntendon * ld); Hd.counts = take(2);
     Hd.total = o;
-    Hand2& H2 = M->hand2;
+    Hand2& H2 = M->ho.H2;
     o = 0;
-    H2.xpos = take(3 * nb); H2.xquat = take(4 * nb); H2.xmat = take(9 * nb); H2.xipos = take(3 * nb); H2.scom = take(3 * nb);
-    H2.cinert = take(10 * nb); H2.cdof = take(6 * nv); H2.cdofdot = take(6 * nv); H2.cvel = take(6 * nb);
-    H2.con = take(m.nconmax * CON_STRIDE);
+#define TAKE_H2(f, n) H2.f = take(n);
+    HAND2_FIELDS(TAKE_H2)
+#undef TAKE_H2
     H2.total = o;
-    auto pick = [](size_t per_env) { int e = (int)((227 * 1024 - 64) / (per_env ? per_env : 1)); return e > 8 ? 8 : e; };   // 64: CTA scratch of the bucket compaction
+    auto pick = [](size_t per_env) { int e = (int)((SMEM_MAX - 64) / (per_env ? per_env : 1)); return e > 8 ? 8 : e; };   // 64: CTA scratch of the bucket compaction
     // several small CTAs per SM: no phase barriers in the split kernels
     // position kernels: CTAs of up to 5 phase-aligned warps, two CTAs per SM when they fit
     M->epb_pos = pick(M->smem_pos) > 5 ? 5 : pick(M->smem_pos);
-    // one 5-warp CTA per SM and room for more warps: the `big` kernels (up to 7 warps, __launch_bounds__(224, 1))
+    // one 5-warp CTA per SM and room for more warps: the POS_BIG kernels (up to 7 warps, __launch_bounds__(224, 1))
     M->pos_big = 0;
-    if (2 * 5 * M->smem_pos + 2 * 64 > 227 * 1024 && pick(M->smem_pos) > 5) { M->pos_big = 1; M->epb_pos = pick(M->smem_pos) > 7 ? 7 : pick(M->smem_pos); }
+    if (2 * 5 * M->smem_pos + 2 * 64 > SMEM_MAX && pick(M->smem_pos) > 5) { M->pos_big = 1; M->epb_pos = pick(M->smem_pos) > 7 ? 7 : pick(M->smem_pos); }
     const int v = M->hooks.epb_pos;
     if (v >= 1 && v <= pick(M->smem_pos) && v <= (M->pos_big ? 7 : 5)) M->epb_pos = v;   // __launch_bounds__(160, ..)
   }
 }
+
+// one field of the compiled-model blob on the host: its first element and its length
+template <class T> struct HostField { const T* p; int n; };
+struct HostModel {
+#define HOST_I(name) HostField<int> name;
+#define HOST_R(name) HostField<double> name;
+  B200MJ_MODEL_FIELDS(HOST_I, HOST_R)
+#undef HOST_I
+#undef HOST_R
+};
+#define COUNT_FIELD(name) + 1
+static const int NFIELDS = 0 B200MJ_MODEL_FIELDS(COUNT_FIELD, COUNT_FIELD);
+#undef COUNT_FIELD
 
 extern "C" {
 
@@ -3213,7 +3186,7 @@ int b200mj_describe(const b200mj_model* M, char* buf, int n) {
   if (!M || !buf || n <= 0) return -1;
   int w = snprintf(buf, n, "{\"fused_workspace_bytes\": %zu, \"fused_envs_per_cta\": %d, \"pos_workspace_bytes\": %zu, \"pos_envs_per_cta\": %d, "
                    "\"handover_bytes_per_env\": %zu, \"acc_buckets\": [", M->smem_per_env, M->envs_per_block, M->smem_pos, M->epb_pos,
-                   (size_t)(M->hand.total + M->hand2.total) * sizeof(double));
+                   (size_t)(M->ho.H.total + M->ho.H2.total) * sizeof(double));
   for (int b = 0; b < M->nbucket && w < n; b++)
     w += snprintf(buf + w, n - w, "%s{\"rows\": %d, \"workspace_bytes\": %zu, \"last_step_workspace_bytes\": %zu}", b ? ", " : "",
                   M->rows_cap[b], M->smem_acc_b[b], M->smem_accs_b[b]);
@@ -3223,20 +3196,19 @@ int b200mj_describe(const b200mj_model* M, char* buf, int n) {
 
 int b200mj_model_create(const int32_t* idata, int ni, const double* rdata, int nr, b200mj_model** out) {
   if (!idata || !rdata || !out || ni <= 0 || nr <= 0) return -1;
-  {   // the blob starts with one (offset, length) pair per field of b200mj_model_fields.h: refuse a malformed directory
-    int nfields = 0;
-#define CNT(name) nfields++;
-    B200MJ_MODEL_FIELDS(CNT, CNT)
-#undef CNT
-    if (ni < 2 * nfields) return -1;
-    int k = 0; bool bad = false;
-#define CHK_I(name) { long off = idata[2*k], len = idata[2*k+1]; if (off < 2 * nfields || len < 0 || off + len > ni) bad = true; k++; }
-#define CHK_R(name) { long off = idata[2*k], len = idata[2*k+1]; if (off < 0 || len < 0 || off + len > nr) bad = true; k++; }
-    B200MJ_MODEL_FIELDS(CHK_I, CHK_R)
-#undef CHK_I
-#undef CHK_R
-    if (bad) return -1;
-  }
+  // the blob starts with one (offset, length) pair per field of b200mj_model_fields.h: refuse a malformed directory,
+  // else locate every field on the host
+  if (ni < 2 * NFIELDS) return -1;
+  HostModel h;
+  int k = 0;
+#define LOCATE(name, base, lo, hi) { const long off = idata[2 * k], len = idata[2 * k + 1]; k++; \
+    if (off < (lo) || len < 0 || off + len > (hi)) return -1; h.name = {base + off, (int)len}; }
+#define LOCATE_I(name) LOCATE(name, idata, 2 * NFIELDS, ni)
+#define LOCATE_R(name) LOCATE(name, rdata, 0, nr)
+  B200MJ_MODEL_FIELDS(LOCATE_I, LOCATE_R)
+#undef LOCATE_I
+#undef LOCATE_R
+#undef LOCATE
   b200mj_model* M = new b200mj_model();
   memset(M, 0, sizeof(*M));
   if (cudaMalloc(&M->d_idata, (size_t)ni * sizeof(int)) != cudaSuccess) { delete M; return -2; }
@@ -3246,87 +3218,60 @@ int b200mj_model_create(const int32_t* idata, int ni, const double* rdata, int n
     cudaFree(M->d_idata); cudaFree(M->d_rdata); delete M; return -2;
   }
   DevModel& m = M->dm;
-  int k = 0;
-  const int *h_sizes = nullptr, *h_opti = nullptr; const double* h_optr = nullptr;
-  const int *h_condim = nullptr, *h_sens_type = nullptr; const double *h_fl = nullptr, *h_damp = nullptr;
-  int n_condim = 0, n_sens = 0, n_fl = 0;
-#define SET_I(name) { int off = idata[2*k], len = idata[2*k+1]; m.name = M->d_idata + off; \
-    if (!strcmp(#name, "sizes")) h_sizes = idata + off; if (!strcmp(#name, "opt_int")) h_opti = idata + off; \
-    if (!strcmp(#name, "geom_condim")) { h_condim = idata + off; n_condim = len; } \
-    if (!strcmp(#name, "sensor_type")) { h_sens_type = idata + off; n_sens = len; } k++; }
-#define SET_R(name) { int off = idata[2*k], len = idata[2*k+1]; m.name = M->d_rdata + off; \
-    if (!strcmp(#name, "opt_real")) h_optr = rdata + off; \
-    if (!strcmp(#name, "dof_frictionloss")) { h_fl = rdata + off; n_fl = len; } if (!strcmp(#name, "dof_damping")) h_damp = rdata + off; k++; }
-  B200MJ_MODEL_FIELDS(SET_I, SET_R)
-#undef SET_I
-#undef SET_R
-  m.nq = h_sizes[BMJ_NQ]; m.nv = h_sizes[BMJ_NV]; m.nu = h_sizes[BMJ_NU]; m.na = h_sizes[BMJ_NA]; m.nbody = h_sizes[BMJ_NBODY];
-  m.njnt = h_sizes[BMJ_NJNT]; m.ngeom = h_sizes[BMJ_NGEOM]; m.nsite = h_sizes[BMJ_NSITE]; m.ntendon = h_sizes[BMJ_NTENDON];
-  m.neq = h_sizes[BMJ_NEQ]; m.nsensor = h_sizes[BMJ_NSENSOR]; m.nsensordata = h_sizes[BMJ_NSENSORDATA];
-  m.npair = h_sizes[BMJ_NPAIR]; m.nlevel = h_sizes[BMJ_NLEVEL]; m.nconmax = h_sizes[BMJ_NCONMAX]; m.njmax = h_sizes[BMJ_NJMAX];
+#define DEV_I(name) m.name = M->d_idata + (h.name.p - idata);
+#define DEV_R(name) m.name = M->d_rdata + (h.name.p - rdata);
+  B200MJ_MODEL_FIELDS(DEV_I, DEV_R)
+#undef DEV_I
+#undef DEV_R
+  const int* sz = h.sizes.p; const int* opti = h.opt_int.p; const double* optr = h.opt_real.p;
+  m.nq = sz[BMJ_NQ]; m.nv = sz[BMJ_NV]; m.nu = sz[BMJ_NU]; m.na = sz[BMJ_NA]; m.nbody = sz[BMJ_NBODY];
+  m.njnt = sz[BMJ_NJNT]; m.ngeom = sz[BMJ_NGEOM]; m.nsite = sz[BMJ_NSITE]; m.ntendon = sz[BMJ_NTENDON];
+  m.neq = sz[BMJ_NEQ]; m.nsensor = sz[BMJ_NSENSOR]; m.nsensordata = sz[BMJ_NSENSORDATA];
+  m.npair = sz[BMJ_NPAIR]; m.nlevel = sz[BMJ_NLEVEL]; m.nconmax = sz[BMJ_NCONMAX]; m.njmax = sz[BMJ_NJMAX];
   m.ldv = m.nv | 1;
-  m.integrator = h_opti[BMJ_OPT_INTEGRATOR]; m.iterations = h_opti[BMJ_OPT_ITERATIONS]; m.solver = h_opti[BMJ_OPT_SOLVER];
-  m.ls_iterations = h_opti[BMJ_OPT_LS_ITERATIONS]; m.disableflags = h_opti[BMJ_OPT_DISABLEFLAGS];
-  m.timestep = h_optr[BMJ_OPT_TIMESTEP];
-  for (int i = 0; i < 3; i++) m.gravity[i] = h_optr[BMJ_OPT_GRAVITY_X + i];
-  m.tolerance = h_optr[BMJ_OPT_TOLERANCE]; m.ls_tolerance = h_optr[BMJ_OPT_LS_TOLERANCE];
-  m.impratio = h_optr[BMJ_OPT_IMPRATIO]; m.meaninertia = h_optr[BMJ_OPT_MEANINERTIA];
+  m.integrator = opti[BMJ_OPT_INTEGRATOR]; m.iterations = opti[BMJ_OPT_ITERATIONS]; m.solver = opti[BMJ_OPT_SOLVER];
+  m.ls_iterations = opti[BMJ_OPT_LS_ITERATIONS]; m.disableflags = opti[BMJ_OPT_DISABLEFLAGS];
+  m.timestep = optr[BMJ_OPT_TIMESTEP];
+  for (int i = 0; i < 3; i++) m.gravity[i] = optr[BMJ_OPT_GRAVITY_X + i];
+  m.tolerance = optr[BMJ_OPT_TOLERANCE]; m.ls_tolerance = optr[BMJ_OPT_LS_TOLERANCE];
+  m.impratio = optr[BMJ_OPT_IMPRATIO]; m.meaninertia = optr[BMJ_OPT_MEANINERTIA];
   m.any_damping = 0;
-  for (int i = 0; i < m.nv; i++) if (h_damp[i] > 0) m.any_damping = 1;
+  for (int i = 0; i < m.nv; i++) if (h.dof_damping.p[i] > 0) m.any_damping = 1;
   m.acc_sensors = 0;
-  for (int i = 0; i < n_sens; i++) { int t = h_sens_type[i]; if (t == BMJ_SENS_ACCELEROMETER || t == BMJ_SENS_FORCE || t == BMJ_SENS_TORQUE) m.acc_sensors = 1; }
-  bool unsupported = m.nv > 64 || (h_opti[BMJ_OPT_SOLVER] != BMJ_SOL_NEWTON && h_opti[BMJ_OPT_SOLVER] != BMJ_SOL_PGS) || h_opti[BMJ_OPT_CONE] != 0 ||
+  for (int i = 0; i < h.sensor_type.n; i++) { int t = h.sensor_type.p[i]; if (t == BMJ_SENS_ACCELEROMETER || t == BMJ_SENS_FORCE || t == BMJ_SENS_TORQUE) m.acc_sensors = 1; }
+  bool unsupported = m.nv > 64 || (opti[BMJ_OPT_SOLVER] != BMJ_SOL_NEWTON && opti[BMJ_OPT_SOLVER] != BMJ_SOL_PGS) || opti[BMJ_OPT_CONE] != 0 ||
                      (m.integrator != BMJ_INT_EULER && m.integrator != BMJ_INT_RK4);
-  for (int i = 0; i < n_condim; i++) if (h_condim[i] != 1 && h_condim[i] != 3) unsupported = true;
-  {   // geom types without a narrow-phase function here (height fields, meshes) must not slip through as contact-free geoms
-    int kk = 0; const int* h_gt = nullptr; int n_gt = 0;
-#define GT_I(name) if (!strcmp(#name, "geom_type")) { h_gt = idata + idata[2 * kk]; n_gt = idata[2 * kk + 1]; } kk++;
-#define GT_R(name) kk++;
-    B200MJ_MODEL_FIELDS(GT_I, GT_R)
-#undef GT_I
-#undef GT_R
-    for (int i = 0; i < n_gt; i++) if (h_gt[i] == BMJ_GEOM_HFIELD || h_gt[i] >= BMJ_GEOM_MESH) unsupported = true;
-  }
-  for (int i = 0; i < n_fl; i++) if (h_fl[i] != 0) unsupported = true;
+  for (int i = 0; i < h.geom_condim.n; i++) if (h.geom_condim.p[i] != 1 && h.geom_condim.p[i] != 3) unsupported = true;
+  // geom types without a narrow-phase function here (height fields, meshes) must not slip through as contact-free geoms
+  for (int i = 0; i < h.geom_type.n; i++) if (h.geom_type.p[i] == BMJ_GEOM_HFIELD || h.geom_type.p[i] >= BMJ_GEOM_MESH) unsupported = true;
+  for (int i = 0; i < h.dof_frictionloss.n; i++) if (h.dof_frictionloss.p[i] != 0) unsupported = true;
   if (unsupported) { b200mj_model_destroy(M); return -3; }
+  // does any candidate pair reach the convex routines (see narrowphase<CVX>)? If not the position kernels are the primitive-only builds.
+  M->convex_pairs = 0;
+  for (int p = 0; p < m.npair; p++) {
+    const int t1 = h.geom_type.p[h.pair_geom1.p[p]], t2 = h.geom_type.p[h.pair_geom2.p[p]];
+    const bool analytic = t1 == BMJ_GEOM_PLANE || (t1 == BMJ_GEOM_SPHERE && (t2 == BMJ_GEOM_SPHERE || t2 == BMJ_GEOM_CAPSULE || t2 == BMJ_GEOM_BOX)) ||
+                          (t1 == BMJ_GEOM_CAPSULE && t2 == BMJ_GEOM_CAPSULE);
+    if (!analytic) M->convex_pairs = 1;
+  }
   {   // actuator moment arms by dof (constant for joint and fixed-tendon transmissions)
-    struct HF {
-#define HF_I(name) const int* name;
-#define HF_R(name) const double* name;
-      B200MJ_MODEL_FIELDS(HF_I, HF_R)
-#undef HF_I
-#undef HF_R
-    } hf;
-    int kk = 0;
-#define HS_I(name) hf.name = idata + idata[2 * kk]; kk++;
-#define HS_R(name) hf.name = rdata + idata[2 * kk]; kk++;
-    B200MJ_MODEL_FIELDS(HS_I, HS_R)
-#undef HS_I
-#undef HS_R
-    // does any candidate pair reach the convex routines (see narrowphase<CVX>)? If not the position kernels are the primitive-only builds.
-    M->convex_pairs = 0;
-    for (int p = 0; p < m.npair; p++) {
-      const int t1 = hf.geom_type[hf.pair_geom1[p]], t2 = hf.geom_type[hf.pair_geom2[p]];
-      const bool analytic = t1 == BMJ_GEOM_PLANE || (t1 == BMJ_GEOM_SPHERE && (t2 == BMJ_GEOM_SPHERE || t2 == BMJ_GEOM_CAPSULE || t2 == BMJ_GEOM_BOX)) ||
-                            (t1 == BMJ_GEOM_CAPSULE && t2 == BMJ_GEOM_CAPSULE);
-      if (!analytic) M->convex_pairs = 1;
-    }
     const int nv = m.nv, nu = m.nu;
     int* adr = new int[nv + 1];
     int* ids = new int[(size_t)nv * (nu > 0 ? nu : 1)];
     double* coef = new double[(size_t)nv * (nu > 0 ? nu : 1)];
+    const int* jnt_dofadr = h.jnt_dofadr.p;
     int n = 0;
     for (int i = 0; i < nv; i++) {
       adr[i] = n;
       for (int a = 0; a < nu; a++) {
         double mom = 0; bool any = false;
-        const double gear = hf.actuator_gear[a];
-        if (hf.actuator_trntype[a] == BMJ_TRN_JOINT) { if (hf.jnt_dofadr[hf.actuator_trnid[a]] == i) { mom = gear; any = true; } }
+        const double gear = h.actuator_gear.p[a];
+        if (h.actuator_trntype.p[a] == BMJ_TRN_JOINT) { if (jnt_dofadr[h.actuator_trnid.p[a]] == i) { mom = gear; any = true; } }
         else {
-          const int t = hf.actuator_trnid[a];
+          const int t = h.actuator_trnid.p[a];
           double tj = 0;
-          for (int w = hf.tendon_adr[t]; w < hf.tendon_adr[t] + hf.tendon_num[t]; w++)
-            if (hf.jnt_dofadr[hf.wrap_objid[w]] == i) { tj += hf.wrap_prm[w]; any = true; }
+          for (int w = h.tendon_adr.p[t]; w < h.tendon_adr.p[t] + h.tendon_num.p[t]; w++)
+            if (jnt_dofadr[h.wrap_objid.p[w]] == i) { tj += h.wrap_prm.p[w]; any = true; }
           mom = gear * tj;
         }
         if (any) { ids[n] = a; coef[n] = mom; n++; }
@@ -3344,8 +3289,8 @@ int b200mj_model_create(const int32_t* idata, int ni, const double* rdata, int n
     m.dof_act_adr = M->d_xi; m.dof_act_id = M->d_xi + nv + 1; m.dof_act_coef = M->d_xr;
   }
   read_test_hooks(M);
-  M->nkey = h_sizes[BMJ_NKEY];
-  M->tn_nv = (M->hooks.tn && tn_kernel(m.nv, false)) ? m.nv : 0;
+  M->nkey = sz[BMJ_NKEY];
+  M->tn_nv = (M->hooks.tn && acc_kernel_for(m.nv, false)) ? m.nv : 0;
   build_layout(M);
   if (M->envs_per_block < 1) { b200mj_model_destroy(M); return -4; }
   for (int g = 0; g < 2; g++) {
@@ -3355,20 +3300,7 @@ int b200mj_model_create(const int32_t* idata, int ni, const double* rdata, int n
   }
   cudaEventCreateWithFlags(&M->ev_fork, cudaEventDisableTiming);
   M->streams_ok = 1;
-  cudaFuncSetAttribute(b200mj_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(b200mj_step_prim_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(b200mj_pos_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(b200mj_acc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(b200mj_acclast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(b200mj_posfinal_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(b200mj_pos_prim_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(b200mj_posfinal_prim_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(b200mj_pos_big_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(b200mj_posfinal_big_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  if (M->tn_nv) {
-    cudaFuncSetAttribute(tn_kernel(M->tn_nv, false), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    cudaFuncSetAttribute(tn_kernel(M->tn_nv, true), cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  }
+  allow_shared_memory(M);
   *out = M;
   return 0;
 }
@@ -3379,8 +3311,8 @@ void b200mj_model_destroy(b200mj_model* M) {
   if (M->d_xi) cudaFree(M->d_xi);
   if (M->d_xr) cudaFree(M->d_xr);
   if (M->d_varid) cudaFree(M->d_varid);
-  if (M->d_hand) cudaFree(M->d_hand);
-  if (M->d_hand2) cudaFree(M->d_hand2);
+  if (M->ho.rows) cudaFree(M->ho.rows);
+  if (M->ho.rows2) cudaFree(M->ho.rows2);
   if (M->d_bcount) cudaFree(M->d_bcount);
   if (M->d_blist) cudaFree(M->d_blist);
   if (M->streams_ok) {
@@ -3404,10 +3336,11 @@ int b200mj_model_set_capacity(b200mj_model* M, int nconmax, int njmax) {
   if (!M || nconmax < 0 || njmax < 0) return -1;
   M->dm.nconmax = nconmax; M->dm.njmax = njmax;
   build_layout(M);
+  allow_shared_memory(M);
   // the handover rows are sized by the layout: drop them, the next b200mj_step allocates for the new capacities
-  if (M->d_hand) cudaFree(M->d_hand);
-  if (M->d_hand2) cudaFree(M->d_hand2);
-  M->d_hand = M->d_hand2 = nullptr; M->hand_batch = 0; M->reuse_ok = 0;
+  if (M->ho.rows) cudaFree(M->ho.rows);
+  if (M->ho.rows2) cudaFree(M->ho.rows2);
+  M->ho.rows = M->ho.rows2 = nullptr; M->hand_batch = 0; M->reuse_ok = 0;
   return M->envs_per_block < 1 ? -4 : 0;
 }
 
@@ -3467,7 +3400,7 @@ static int launch(const b200mj_model* M, const b200mj_io* io, int batch, int nst
   int epb = M->envs_per_block;
   int grid = (batch + epb - 1) / epb;
   const size_t smem = M->smem_per_env * epb;
-  B200MJ_LAUNCH((M->convex_pairs ? b200mj_step_kernel : b200mj_step_prim_kernel), grid, 32 * epb, smem, (cudaStream_t)stream, M->dm, M->lay, *io, batch, nstep, flags, mode, extra, env_mask);
+  B200MJ_LAUNCH(step_kernel_for(M), grid, 32 * epb, smem, (cudaStream_t)stream, M->dm, M->lay, *io, batch, nstep, flags, mode, extra, env_mask);
   g_launches++;
   return cudaGetLastError() == cudaSuccess ? 0 : -5;
 }
@@ -3479,15 +3412,15 @@ int b200mj_step(const b200mj_model* Mc, const b200mj_io* io, int batch, int nste
   // non-legacy ordering, qfrc/xfrc_applied) runs through the fused kernel.
   bool can_split = M->hooks.split && nstep >= 1 && (flags & B200MJ_STEP_LEGACY) && M->dm.integrator == BMJ_INT_EULER &&
                    M->dm.solver == BMJ_SOL_NEWTON &&
-                   !io->qfrc_applied && !io->xfrc_applied && M->epb_pos >= 1 && M->smem_accs_b[M->nbucket - 1] <= 227 * 1024 &&
+                   !io->qfrc_applied && !io->xfrc_applied && M->epb_pos >= 1 && M->smem_accs_b[M->nbucket - 1] <= SMEM_MAX &&
                    io->qpos && io->qvel && (M->dm.na == 0 || io->act);
   if (!can_split) return launch(M, io, batch, nstep, flags, MODE_STEP, 0, stream);
   if (M->hand_batch < batch) {
-    if (M->d_hand) cudaFree(M->d_hand);
-    if (M->d_hand2) cudaFree(M->d_hand2);
-    M->d_hand = M->d_hand2 = nullptr; M->hand_batch = 0; M->reuse_ok = 0;
-    if (cudaMalloc(&M->d_hand, (size_t)(batch + SHADOW_ROWS) * M->hand.total * sizeof(double)) != cudaSuccess) return -2;
-    if (cudaMalloc(&M->d_hand2, (size_t)(batch + SHADOW_ROWS) * M->hand2.total * sizeof(double)) != cudaSuccess) return -2;
+    if (M->ho.rows) cudaFree(M->ho.rows);
+    if (M->ho.rows2) cudaFree(M->ho.rows2);
+    M->ho.rows = M->ho.rows2 = nullptr; M->hand_batch = 0; M->reuse_ok = 0;
+    if (cudaMalloc(&M->ho.rows, (size_t)(batch + SHADOW_ROWS) * M->ho.H.total * sizeof(double)) != cudaSuccess) return -2;
+    if (cudaMalloc(&M->ho.rows2, (size_t)(batch + SHADOW_ROWS) * M->ho.H2.total * sizeof(double)) != cudaSuccess) return -2;
     if (M->d_bcount) cudaFree(M->d_bcount);
     if (M->d_blist) cudaFree(M->d_blist);
     M->d_bcount = M->d_blist = nullptr;
@@ -3499,7 +3432,7 @@ int b200mj_step(const b200mj_model* Mc, const b200mj_io* io, int batch, int nste
   cudaStream_t st = (cudaStream_t)stream;
   const bool want_sens = (flags & B200MJ_STEP_SENSORS) != 0;
   // Every physics step is split; the last one uses the sensor-carrying acceleration kernel and the trailing mj_step1 is
-  // the `posfinal` kernel.
+  // the FINAL position kernel.
   // B200MJ_STEP_REUSE_POS: the previous call's trailing mj_step1 wrote this state's handover rows already
   // (the trailing mj_step1 dumps what the acceleration-stage sensors need only when the call had one physics step: a
   // call whose first step is also its last must then find that dump, or recompute the position stage)
@@ -3540,8 +3473,8 @@ int b200mj_step(const b200mj_model* Mc, const b200mj_io* io, int batch, int nste
       const bool last = s == nstep - 1;
       if (!(reuse && s == 0)) {
         const Compact cp = compact();
-        B200MJ_LAUNCH((M->pos_big ? b200mj_pos_big_kernel : M->convex_pairs ? b200mj_pos_kernel : b200mj_pos_prim_kernel), gp, 32 * M->epb_pos, M->smem_pos * M->epb_pos + 64, sm, M->dm, M->lay_pos, M->hand, M->hand2, *io, M->d_hand, M->d_hand2,
-                                                                                 e1, 0, flags, last && want_sens, e0, cp);
+        B200MJ_LAUNCH(pos_kernel_for(M, false), gp, 32 * M->epb_pos, M->smem_pos * M->epb_pos + 64, sm, M->dm, M->lay_pos, M->ho, *io,
+                      e1, flags, last && want_sens, e0, cp);
         g_launches++;
       }
       if (M->nbucket > 1) cudaEventRecord(M->ev_pos[g], sm);
@@ -3549,25 +3482,24 @@ int b200mj_step(const b200mj_model* Mc, const b200mj_io* io, int batch, int nste
         cudaStream_t sb = b == 0 ? sm : M->gaux[g][b];     // buckets are independent: let them share the SMs
         if (b > 0) cudaStreamWaitEvent(sb, M->ev_pos[g], 0);
         const size_t ws = (last ? M->smem_accs_b[b] : M->smem_acc_b[b]);
-        // warps per CTA: as many as fit 227 KB, at most acc_warps
+        // warps per CTA: as many as fit SMEM_MAX, at most acc_warps
         const int want = M->tn_nv ? M->hooks.acc_warps : 8;      // runtime-size kernels (__launch_bounds__(256)): whatever fills the SM
-        int cap = (int)((227 * 1024) / ws); if (cap > want) cap = want; if (M->tn_nv && cap > 4) cap = 4; if (cap < 1) cap = 1;
-        // as many resident warps per SM as 227 KB allow (CMU corridor, 37 KB per warp: two CTAs of 3 instead of one of 4); ties: the larger CTA
+        int cap = (int)(SMEM_MAX / ws); if (cap > want) cap = want; if (M->tn_nv && cap > 4) cap = 4; if (cap < 1) cap = 1;
+        // as many resident warps per SM as SMEM_MAX allows (CMU corridor, 37 KB per warp: two CTAs of 3 instead of one of 4); ties: the larger CTA
         int wpc = 1, best = 0;
-        for (int w = cap; w >= 1; w--) { const int res = (int)((227 * 1024) / ((w * ws) + 1024)) * w; if (res > best) { best = res; wpc = w; } }
+        for (int w = cap; w >= 1; w--) { const int res = (int)(SMEM_MAX / ((w * ws) + 1024)) * w; if (res > best) { best = res; wpc = w; } }
         const int grid = (cnt + wpc - 1) / wpc;
         const int* bl = glist + (size_t)b * M->hand_batch;
         const Lay& la = last ? M->lay_accs_b[b] : M->lay_acc_b[b];
-        acc_kernel_fn fn = M->tn_nv ? tn_kernel(M->tn_nv, last) : last ? (acc_kernel_fn)b200mj_acclast_kernel : (acc_kernel_fn)b200mj_acc_kernel;
-        B200MJ_LAUNCH(fn, grid, 32 * wpc, ws * wpc, sb, M->dm, la, M->hand, M->hand2, *io, M->d_hand, M->d_hand2, 0, s == 0, flags, gcount + b, bl);
+        B200MJ_LAUNCH(acc_kernel_for(M->tn_nv, last), grid, 32 * wpc, ws * wpc, sb, M->dm, la, M->ho, *io, s == 0, flags, gcount + b, bl);
         if (b > 0) cudaEventRecord(M->ev_acc[g][b], sb);
         g_launches++;
       }
       for (int b = 1; b < M->nbucket; b++) cudaStreamWaitEvent(sm, M->ev_acc[g][b], 0);   // join after the main-stream bucket is queued
     }
     const Compact cp = compact();      // the lists of the next call's first physics step
-    B200MJ_LAUNCH((M->pos_big ? b200mj_posfinal_big_kernel : M->convex_pairs ? b200mj_posfinal_kernel : b200mj_posfinal_prim_kernel), gp, 32 * M->epb_pos, M->smem_pos * M->epb_pos + 64, sm, M->dm, M->lay_pos, M->hand, M->hand2, *io, M->d_hand, M->d_hand2,
-                                                                                  e1, 0, flags, want_sens && nstep == 1, e0, cp);
+    B200MJ_LAUNCH(pos_kernel_for(M, true), gp, 32 * M->epb_pos, M->smem_pos * M->epb_pos + 64, sm, M->dm, M->lay_pos, M->ho, *io,
+                  e1, flags, want_sens && nstep == 1, e0, cp);
     g_launches++;
     if (g > 0) { cudaEventRecord(M->ev_join[g], sm); cudaStreamWaitEvent(st, M->ev_join[g], 0); }
   }

@@ -18,8 +18,9 @@ from dm_control_b200.physics import BatchedPhysics
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(os.path.dirname(_HERE))
 _SRC = os.path.join(_ROOT, 'dm_control_b200', 'csrc', 'b200mj.cu')
-_DEPS = [_SRC, os.path.join(_HERE, 'cuda_emu.h'), os.path.join(_ROOT, 'include', 'b200mj.h'),
-         os.path.join(_ROOT, 'include', 'b200mj_model_fields.h')]
+# the kernel source and every header it includes: an edit to any of them rebuilds the emulation library
+_DEPS = [_SRC, os.path.join(_HERE, 'cuda_emu.h')] + [os.path.join(_ROOT, 'include', h) for h in
+                                                    ('b200mj.h', 'b200mj_model_fields.h', 'b200mj_convex.h')]
 _SO = os.path.join(_HERE, '_build', 'libb200mj_emu.so')
 _lib = None
 

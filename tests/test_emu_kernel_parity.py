@@ -449,12 +449,10 @@ def test_address_sanitizer_finds_nothing():
   if not os.path.isabs(libasan) or not os.path.exists(libasan):
     pytest.skip('libasan not available')
   so = os.path.join(root, 'tests', 'emu', '_build', 'libb200mj_emu_asan.so')
-  src = os.path.join(root, 'dm_control_b200', 'csrc', 'b200mj.cu')
-  hdr = os.path.join(root, 'tests', 'emu', 'cuda_emu.h')
-  if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(src), os.path.getmtime(hdr)):
+  if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(d) for d in emu._DEPS):
     os.makedirs(os.path.dirname(so), exist_ok=True)
     subprocess.check_call(['g++', '-std=c++20', '-O1', '-g', '-fno-omit-frame-pointer', '-fsanitize=address', '-fPIC', '-shared',
-                           '-pthread', '-x', 'c++', '-DB200MJ_CPU_EMU', '-Wno-unknown-pragmas', '-I' + os.path.dirname(hdr), '-o', so, src])
+                           '-pthread', '-x', 'c++', '-DB200MJ_CPU_EMU', '-Wno-unknown-pragmas', '-I' + emu._HERE, '-o', so, emu._SRC])
   env = dict(os.environ, LD_PRELOAD=libasan, ASAN_OPTIONS='detect_leaks=0:detect_stack_use_after_return=0')
   out = subprocess.run([sys.executable, '-c', _ASAN_SCRIPT, root, so], env=env, capture_output=True, text=True, timeout=900)
   assert 'ERROR: AddressSanitizer' not in out.stderr, out.stderr[-3000:]
