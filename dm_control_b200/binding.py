@@ -8,7 +8,7 @@ The reference binds `mjcf.Element`s; the PyMJCF object model is out of scope her
     `jnt_range` -> `.range`, `actuator_gear` -> `.gear`), data fields by their own name (`xpos`, `qpos`, `qvel`, `ctrl`,
     `sensordata`, `subtree_linvel`, ...), `element_id`;
   * ragged fields resolve through the address tables (`qpos`/`qvel` of a joint, `sensordata` of a sensor);
-  * writes to the STATE through a binding (`qpos qvel act ctrl qacc_warmstart time`) mark the physics dirty, and the
+  * writes to the STATE through a binding (the fields `physics.DATA_FIELDS` marks STATE) mark the physics dirty, and the
     next read of a DERIVED field through any binding runs `forward()` first — lazily, once
     (mjcf/physics.py:211-237 `_triggers_dirty` / `is_dirty`). Model writes re-upload the model before the next call.
 
@@ -19,16 +19,11 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-_STATE = ('qpos', 'qvel', 'act', 'ctrl', 'qacc_warmstart', 'time')
+from . import index
+from .physics import DATA_FIELDS, STATE
+
 _PREFIX = dict(body='body_', geom='geom_', site='site_', joint='jnt_', actuator='actuator_', sensor='sensor_', tendon='tendon_',
                dof='dof_')
-# data fields addressable per element kind: name -> (row kind, ragged address table or None)
-_DATA = {
-    'body': ('xpos', 'xquat', 'xmat', 'xipos', 'subtree_com', 'subtree_linvel', 'cvel', 'xfrc_applied'),
-    'geom': ('geom_xpos', 'geom_xmat'),
-    'site': ('site_xpos', 'site_xmat'),
-    'actuator': ('ctrl', 'actuator_force'),
-}
 _DATA_ALIAS = {'geom': {'xpos': 'geom_xpos', 'xmat': 'geom_xmat'}, 'site': {'xpos': 'site_xpos', 'xmat': 'site_xmat'},
                'actuator': {'force': 'actuator_force'}}
 
@@ -48,23 +43,17 @@ class Binding:
     object.__setattr__(self, '_tids', torch.as_tensor(ids, device=physics.device))
 
   # ---- helpers ----
-  def _ragged(self, field):
-    """Flat column indices of a ragged data field for the bound elements (or None)."""
-    m, ids = self._p.model, self._ids
-    if self._kind == 'joint' and field in ('qpos', 'qvel', 'qacc', 'qacc_warmstart', 'qfrc_bias', 'qfrc_passive', 'qfrc_actuator', 'qfrc_constraint',
-                                           'qfrc_applied'):
-      qp = field == 'qpos'
-      adr = np.asarray(m.jnt_qposadr if qp else m.jnt_dofadr)
-      width = {0: (7, 6), 1: (4, 3), 2: (1, 1), 3: (1, 1)}
-      cols = [a + k for j in ids for a in [int(adr[j])] for k in range(width[int(m.jnt_type[j])][0 if qp else 1])]
-      return np.array(cols, dtype=np.int64)
-    if self._kind == 'sensor' and field == 'sensordata':
-      adr, dim = np.asarray(m.sensor_adr), np.asarray(m.sensor_dim)
-      return np.array([int(adr[s]) + k for s in ids for k in range(int(dim[s]))], dtype=np.int64)
-    if self._kind == 'actuator' and field == 'act':
-      adr = np.asarray(m.actuator_actadr)
-      return np.array([int(adr[a]) for a in ids if adr[a] >= 0], dtype=np.int64)
-    return None
+  def _index(self, name, field):
+    """(ragged, indices along axis 1 of `data.<field>`) of the bound elements: the columns of their slices of a ragged
+    field (the slices `physics.named` uses), or their rows of a per-element field."""
+    rows = DATA_FIELDS[field].rows if field in DATA_FIELDS else None
+    if rows in index._RAGGED_AXES and index._RAGGED_AXES[rows][0] == self._kind:
+      slices = index._ragged(self._p.model, rows)
+      cols = [c for i in self._ids if slices[i] is not None for c in range(slices[i].start, slices[i].stop)]
+      return True, torch.tensor(cols, dtype=torch.int64, device=self._p.device)
+    if rows == self._kind:
+      return False, self._tids
+    raise AttributeError(f'{name!r} is not a per-{self._kind} data field')
 
   def _data_field(self, name):
     d = self._p.data
@@ -80,16 +69,11 @@ class Binding:
     p = self._p
     field, t = self._data_field(name)
     if t is not None:
-      if field not in _STATE and getattr(p, '_bind_dirty', False):
+      ragged, idx = self._index(name, field)
+      if DATA_FIELDS[field].role != STATE and getattr(p, '_bind_dirty', False):
         p.forward()                              # lazily, once: derived quantities after a state write through a binding
-      cols = self._ragged(field)
-      if cols is not None:
-        return t.index_select(1, torch.as_tensor(cols, device=p.device))
-      if field in _DATA.get(self._kind, ()) or field in ('ctrl',):
-        n = {'body': p.model.nbody, 'geom': p.model.ngeom, 'site': p.model.nsite, 'actuator': p.model.nu}[self._kind]
-        return self._squeeze(t.reshape(p.batch, n, -1).index_select(1, self._tids)).squeeze(-1) if t.numel() // (p.batch * n) == 1 \
-            else self._squeeze(t.reshape(p.batch, n, -1).index_select(1, self._tids))
-      raise AttributeError(f'{name!r} is not a per-{self._kind} data field')
+      out = t.index_select(1, idx)
+      return out if ragged else self._squeeze(out)
     mname = _PREFIX[self._kind] + name
     arr = p.model.fields.get(mname)
     if arr is None:
@@ -104,15 +88,14 @@ class Binding:
     field, t = self._data_field(name)
     if t is not None:
       v = torch.as_tensor(value, dtype=t.dtype, device=p.device)
-      cols = self._ragged(field)
-      if cols is not None:
-        t[:, torch.as_tensor(cols, device=p.device)] = v
+      ragged, idx = self._index(name, field)
+      if ragged:
+        t[:, idx] = v
       else:
-        n = {'body': p.model.nbody, 'geom': p.model.ngeom, 'site': p.model.nsite, 'actuator': p.model.nu}[self._kind]
-        view = t.reshape(p.batch, n, -1)
-        view[:, self._tids] = v.reshape((-1, len(self._ids), view.shape[2])) if v.numel() > view.shape[2] * len(self._ids) or v.dim() >= 2 \
+        view = t.reshape(p.batch, t.shape[1], -1)
+        view[:, idx] = v.reshape((-1, len(self._ids), view.shape[2])) if v.numel() > view.shape[2] * len(self._ids) or v.dim() >= 2 \
             else v.reshape(1, -1, view.shape[2]).expand(p.batch, len(self._ids), view.shape[2])
-      if field in _STATE:
+      if DATA_FIELDS[field].role == STATE:
         p.mark_as_dirty()
         if field != 'ctrl':                      # ctrl does not invalidate position / velocity-stage quantities
           object.__setattr__(p, '_bind_dirty', True)

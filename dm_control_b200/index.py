@@ -11,52 +11,47 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-_COLS = {3: ['x', 'y', 'z'], 4: ['qw', 'qx', 'qy', 'qz'], 9: ['xx', 'xy', 'xz', 'yx', 'yy', 'yz', 'zx', 'zy', 'zz']}
-_RGBA = {'geom_rgba', 'site_rgba', 'mat_rgba'}      # columns r g b a (index.py:103-175 `rgba`); visual tables, Model.vis
-_XYZ = {'body_pos', 'body_ipos', 'body_inertia', 'jnt_pos', 'jnt_axis', 'geom_size', 'geom_pos', 'site_size', 'site_pos',
-        'xpos', 'xipos', 'xanchor', 'xaxis', 'geom_xpos', 'site_xpos', 'subtree_com', 'subtree_linvel'}
-_QUAT = {'body_quat', 'body_iquat', 'geom_quat', 'site_quat', 'xquat'}
-_MAT = {'xmat', 'ximat', 'geom_xmat', 'site_xmat'}
+from .physics import DATA_FIELDS
 
-# field -> kind of its row axis
+_COLS = {'xyz': ['x', 'y', 'z'], 'quat': ['qw', 'qx', 'qy', 'qz'], 'mat': ['xx', 'xy', 'xz', 'yx', 'yy', 'yz', 'zx', 'zy', 'zz'],
+         'rgba': ['r', 'g', 'b', 'a']}
+# field -> kind of its column names; the data fields' come from physics.DATA_FIELDS
+_COL_KIND = {
+    **dict.fromkeys(('body_pos', 'body_ipos', 'body_inertia', 'jnt_pos', 'jnt_axis', 'geom_size', 'geom_pos', 'site_size',
+                     'site_pos'), 'xyz'),
+    **dict.fromkeys(('body_quat', 'body_iquat', 'geom_quat', 'site_quat'), 'quat'),
+    **dict.fromkeys(('geom_rgba', 'site_rgba', 'mat_rgba'), 'rgba'),      # index.py:103-175 `rgba`; visual tables, Model.vis
+    **{n: f.cols for n, f in DATA_FIELDS.items() if f.cols},
+}
+
+# field -> kind of its row axis; the data fields' come from physics.DATA_FIELDS
 _ROW_KIND = {
-    **{f: 'body' for f in ('xpos', 'xquat', 'xmat', 'xipos', 'subtree_com', 'subtree_linvel', 'cvel', 'xfrc_applied',
-                           'body_pos', 'body_quat', 'body_ipos', 'body_iquat', 'body_mass', 'body_inertia',
-                           'body_parentid', 'body_rootid', 'body_subtreemass')},
-    **{f: 'geom' for f in ('geom_xpos', 'geom_xmat', 'geom_size', 'geom_pos', 'geom_quat', 'geom_type', 'geom_bodyid',
-                           'geom_friction', 'geom_rbound', 'geom_condim', 'geom_rgba', 'geom_group')},
-    **{f: 'site' for f in ('site_xpos', 'site_xmat', 'site_pos', 'site_quat', 'site_size', 'site_bodyid', 'site_rgba', 'site_group')},
+    **{f: 'body' for f in ('body_pos', 'body_quat', 'body_ipos', 'body_iquat', 'body_mass', 'body_inertia', 'body_parentid',
+                           'body_rootid', 'body_subtreemass')},
+    **{f: 'geom' for f in ('geom_size', 'geom_pos', 'geom_quat', 'geom_type', 'geom_bodyid', 'geom_friction', 'geom_rbound',
+                           'geom_condim', 'geom_rgba', 'geom_group')},
+    **{f: 'site' for f in ('site_pos', 'site_quat', 'site_size', 'site_bodyid', 'site_rgba', 'site_group')},
     **{f: 'camera' for f in ('cam_pos', 'cam_quat', 'cam_fovy', 'cam_bodyid', 'cam_mode', 'cam_targetbodyid')},
     'mat_rgba': 'material',
     **{f: 'joint' for f in ('jnt_type', 'jnt_range', 'jnt_limited', 'jnt_pos', 'jnt_axis', 'jnt_stiffness', 'jnt_qposadr',
                             'jnt_dofadr', 'jnt_bodyid')},
-    **{f: 'actuator' for f in ('ctrl', 'actuator_force', 'actuator_ctrlrange', 'actuator_gear', 'actuator_ctrllimited')},
-    **{f: 'nq' for f in ('qpos', 'qpos0')},
-    **{f: 'nv' for f in ('qvel', 'qacc', 'qacc_warmstart', 'qfrc_bias', 'qfrc_passive', 'qfrc_actuator', 'qfrc_constraint',
-                         'qfrc_applied', 'dof_damping', 'dof_armature')},
-    'act': 'na', 'sensordata': 'nsensordata',
+    **{f: 'actuator' for f in ('actuator_ctrlrange', 'actuator_gear', 'actuator_ctrllimited')},
+    'qpos0': 'nq', 'dof_damping': 'nv', 'dof_armature': 'nv',
+    **{n: f.rows for n, f in DATA_FIELDS.items() if f.rows},
 }
 
+# ragged axis -> (element kind that owns its slices, address table)
+_RAGGED_AXES = {'nq': ('joint', 'jnt_qposadr'), 'nv': ('joint', 'jnt_dofadr'), 'na': ('actuator', 'actuator_actadr'),
+               'nsensordata': ('sensor', 'sensor_adr')}
 
-def _ragged(model, kind):
-  """name -> slice for the ragged axes (index.py:245-267)."""
-  out = {}
-  if kind == 'nq':
-    adr, names, total = model.jnt_qposadr, model.ordered_names['joint'], model.nq
-  elif kind == 'nv':
-    adr, names, total = model.jnt_dofadr, model.ordered_names['joint'], model.nv
-  elif kind == 'nsensordata':
-    adr, names, total = model.sensor_adr, model.ordered_names['sensor'], model.nsensordata
-  else:   # 'na': singleton per actuator, -1 = none
-    for i, n in enumerate(model.ordered_names['actuator']):
-      a = int(model.actuator_actadr[i])
-      if a >= 0:
-        out[n] = slice(a, a + 1)
-    return out
-  ends = list(adr[1:]) + [total]
-  for n, a, b in zip(names, adr, ends):
-    out[n] = slice(int(a), int(b))
-  return out
+
+def _ragged(model, axis):
+  """Slice of every element along a ragged axis, in element order (index.py:245-267); None for an actuator without an
+  activation (an `na` slice is one column)."""
+  adr = [int(a) for a in getattr(model, _RAGGED_AXES[axis][1])]
+  if axis == 'na':
+    return [slice(a, a + 1) if a >= 0 else None for a in adr]
+  return [slice(a, b) for a, b in zip(adr, adr[1:] + [getattr(model, axis)])]
 
 
 class FieldIndexer:
@@ -65,17 +60,12 @@ class FieldIndexer:
   def __init__(self, name, array, model, batched, on_write=None):
     self._name, self._a, self._batched, self._on_write = name, array, batched, on_write
     kind = _ROW_KIND.get(name)
-    self._ragged = kind in ('nq', 'nv', 'na', 'nsensordata')
-    if kind is None:
-      self._rows = {}
-    elif self._ragged:
-      self._rows = _ragged(model, kind)
+    if kind in _RAGGED_AXES:
+      names = model.ordered_names[_RAGGED_AXES[kind][0]]
+      self._rows = {n: s for n, s in zip(names, _ragged(model, kind)) if s is not None}
     else:
       self._rows = {n: i for i, n in enumerate(model.ordered_names.get(kind, []))}
-    ncol = array.shape[-1] if array.ndim - (1 if batched else 0) >= 2 else 0
-    self._cols = {c: i for i, c in enumerate(_COLS.get(ncol, []))} if (name in _XYZ or name in _QUAT or name in _MAT) else {}
-    if name in _RGBA:
-      self._cols = {'r': 0, 'g': 1, 'b': 2, 'a': 3}
+    self._cols = {c: i for i, c in enumerate(_COLS.get(_COL_KIND.get(name), []))}
 
   def _row_key(self, k):
     if isinstance(k, str):
@@ -151,13 +141,6 @@ class NamedIndexStructs:
   def __init__(self, physics):
     m = physics.model
 
-    def data_get(name):
-      t = getattr(physics.data, name, None)
-      if t is None:
-        return None
-      # [B, nbody*3]-style fields are exposed as [B, nbody, 3] (they are allocated that way already)
-      return t
-
     def model_get(name):
       a = m.fields.get(name)
       if a is None:
@@ -168,5 +151,5 @@ class NamedIndexStructs:
            'geom_quat': 4, 'geom_friction': 3, 'site_pos': 3, 'site_quat': 4, 'site_size': 3, 'jnt_pos': 3, 'jnt_axis': 3,
            'jnt_range': 2, 'actuator_ctrlrange': 2}.get(name)
       return a.reshape(-1, w) if (w and a.ndim == 1) else a
-    self.data = _Struct(data_get, m, True)
+    self.data = _Struct(lambda name: getattr(physics.data, name, None), m, True)
     self.model = _Struct(model_get, m, False)

@@ -14,6 +14,7 @@ from __future__ import annotations
 import contextlib
 import ctypes
 import types
+from typing import NamedTuple
 
 import numpy as np
 import torch
@@ -42,6 +43,66 @@ def action_spec(physics):
   return lo.astype(np.float64), hi.astype(np.float64)
 
 
+STATE, APPLIED, OUTPUT = 'state', 'applied', 'output'
+
+
+class DataField(NamedTuple):
+  """One batched `data.<name>` field, a `b200mj_io` pointer (include/b200mj.h)."""
+  name: str
+  dims: tuple        # per-environment shape: model sizes by name ('nbody') and constants
+  dtype: torch.dtype
+  rows: str | None   # row axis: element kind ('body', 'geom', 'site', 'actuator') or ragged axis ('nq', 'nv', 'na', 'nsensordata')
+  cols: str | None   # column names of index.py: 'xyz', 'quat' or 'mat'
+  role: str          # STATE: uploaded and downloaded by every call; APPLIED: state once enable_applied_forces(); OUTPUT
+
+  def shape(self, m):
+    return tuple(getattr(m, d) if isinstance(d, str) else d for d in self.dims)
+
+
+_F8, _I4 = torch.float64, torch.int32
+# every b200mj_io pointer in the header's order, except var_geom_pos / var_geom_size (set_variable_geoms)
+DATA_FIELDS = {f.name: f for f in (DataField(*row) for row in (
+    ('qpos', ('nq',), _F8, 'nq', None, STATE),
+    ('qvel', ('nv',), _F8, 'nv', None, STATE),
+    ('act', ('na',), _F8, 'na', None, STATE),
+    ('qacc_warmstart', ('nv',), _F8, 'nv', None, STATE),
+    ('time', (), _F8, None, None, STATE),
+    ('ctrl', ('nu',), _F8, 'actuator', None, STATE),
+    ('qfrc_applied', ('nv',), _F8, 'nv', None, APPLIED),
+    ('xfrc_applied', ('nbody', 6), _F8, 'body', None, APPLIED),
+    ('xpos', ('nbody', 3), _F8, 'body', 'xyz', OUTPUT),
+    ('xquat', ('nbody', 4), _F8, 'body', 'quat', OUTPUT),
+    ('xmat', ('nbody', 9), _F8, 'body', 'mat', OUTPUT),
+    ('xipos', ('nbody', 3), _F8, 'body', 'xyz', OUTPUT),
+    ('geom_xpos', ('ngeom', 3), _F8, 'geom', 'xyz', OUTPUT),
+    ('geom_xmat', ('ngeom', 9), _F8, 'geom', 'mat', OUTPUT),
+    ('site_xpos', ('nsite', 3), _F8, 'site', 'xyz', OUTPUT),
+    ('site_xmat', ('nsite', 9), _F8, 'site', 'mat', OUTPUT),
+    ('subtree_com', ('nbody', 3), _F8, 'body', 'xyz', OUTPUT),
+    ('subtree_linvel', ('nbody', 3), _F8, 'body', 'xyz', OUTPUT),
+    ('cvel', ('nbody', 6), _F8, 'body', None, OUTPUT),
+    ('sensordata', ('nsensordata',), _F8, 'nsensordata', None, OUTPUT),
+    ('qM', ('nv', 'nv'), _F8, None, None, OUTPUT),
+    ('qfrc_bias', ('nv',), _F8, 'nv', None, OUTPUT),
+    ('qfrc_passive', ('nv',), _F8, 'nv', None, OUTPUT),
+    ('qacc', ('nv',), _F8, 'nv', None, OUTPUT),
+    ('qfrc_actuator', ('nv',), _F8, 'nv', None, OUTPUT),
+    ('actuator_force', ('nu',), _F8, 'actuator', None, OUTPUT),
+    ('qfrc_constraint', ('nv',), _F8, 'nv', None, OUTPUT),
+    ('efc_force', ('njmax',), _F8, None, None, OUTPUT),
+    ('ncon', (), _I4, None, None, OUTPUT),
+    ('contact_geom', ('nconmax', 2), _I4, None, None, OUTPUT),
+    ('contact_efc_address', ('nconmax',), _I4, None, None, OUTPUT),
+    ('contact_dist', ('nconmax',), _F8, None, None, OUTPUT),
+    ('contact_pos', ('nconmax', 3), _F8, None, None, OUTPUT),
+    ('contact_frame', ('nconmax', 9), _F8, None, None, OUTPUT),
+    ('nefc', (), _I4, None, None, OUTPUT),
+    ('solver_niter', (), _I4, None, None, OUTPUT),
+    ('warning', (8,), _I4, None, None, OUTPUT)))}    # always allocated: check_invalid_state reads it
+STATE_FIELDS = tuple(n for n, f in DATA_FIELDS.items() if f.role == STATE)
+APPLIED_FIELDS = tuple(n for n, f in DATA_FIELDS.items() if f.role == APPLIED)
+
+
 class _Data:
   """Batched mjData slice: `[B, ...]` torch tensors, MuJoCo field names."""
 
@@ -51,24 +112,9 @@ class BatchedPhysics:
 
   legacy_step = True   # reference default: rl/control.py:209
 
-  # (name, per-env shape as a function of model, dtype)
-  _FIELDS = (
-      ('qpos', lambda m: (m.nq,)), ('qvel', lambda m: (m.nv,)), ('act', lambda m: (m.na,)),
-      ('qacc_warmstart', lambda m: (m.nv,)), ('time', lambda m: ()), ('ctrl', lambda m: (m.nu,)),
-      ('qfrc_applied', lambda m: (m.nv,)), ('xfrc_applied', lambda m: (m.nbody, 6)),
-      ('xpos', lambda m: (m.nbody, 3)), ('xquat', lambda m: (m.nbody, 4)), ('xmat', lambda m: (m.nbody, 9)),
-      ('xipos', lambda m: (m.nbody, 3)), ('geom_xpos', lambda m: (m.ngeom, 3)), ('geom_xmat', lambda m: (m.ngeom, 9)),
-      ('site_xpos', lambda m: (m.nsite, 3)), ('site_xmat', lambda m: (m.nsite, 9)),
-      ('subtree_com', lambda m: (m.nbody, 3)), ('subtree_linvel', lambda m: (m.nbody, 3)),
-      ('cvel', lambda m: (m.nbody, 6)), ('sensordata', lambda m: (m.nsensordata,)), ('qM', lambda m: (m.nv, m.nv)),
-      ('qfrc_bias', lambda m: (m.nv,)), ('qfrc_passive', lambda m: (m.nv,)), ('qacc', lambda m: (m.nv,)),
-      ('qfrc_actuator', lambda m: (m.nv,)), ('actuator_force', lambda m: (m.nu,)),
-      ('qfrc_constraint', lambda m: (m.nv,)), ('efc_force', lambda m: (m.njmax,)),
-      ('contact_dist', lambda m: (m.nconmax,)), ('contact_pos', lambda m: (m.nconmax, 3)),
-      ('contact_frame', lambda m: (m.nconmax, 9)))
-  _INT_FIELDS = (('ncon', lambda m: ()), ('contact_geom', lambda m: (m.nconmax, 2)),
-                 ('contact_efc_address', lambda m: (m.nconmax,)), ('nefc', lambda m: ()),
-                 ('solver_niter', lambda m: ()), ('warning', lambda m: (8,)))
+  # (name, per-environment shape as a function of the model) of the float64 and of the int32 fields
+  _FIELDS = tuple((n, f.shape) for n, f in DATA_FIELDS.items() if f.dtype == _F8)
+  _INT_FIELDS = tuple((n, f.shape) for n, f in DATA_FIELDS.items() if f.dtype == _I4)
 
   def __init__(self, model, batch=1, device=None, outputs='all', sensors=True, full_final=True, nconmax=None,
                njmax=None):
@@ -102,27 +148,17 @@ class BatchedPhysics:
     self._pos_current = False
     self._handle = ctypes.c_void_p()
     self._upload_model()
-    m, B = model, self.batch
     self.data = _Data()
-    state_names = ('qpos', 'qvel', 'act', 'qacc_warmstart', 'time', 'ctrl', 'qfrc_applied', 'xfrc_applied')
-    want = None if outputs == 'all' else set(outputs) | set(state_names) | {'warning'}
     self._io = _lib.IO()
     self._applied_dirty = False
     self._applied_on = False
-    for name, shp in self._FIELDS:
-      if want is not None and name not in want:
-        continue
-      if name in ('qfrc_applied', 'xfrc_applied'):
-        continue        # allocated by enable_applied_forces(): writing to them before that must fail loudly, not be ignored
-      t = torch.zeros((B,) + tuple(shp(m)), dtype=torch.float64, device=self.device)
-      setattr(self.data, name, t)
-    for name, shp in self._INT_FIELDS:
-      if want is not None and name not in want:
-        continue
-      t = torch.zeros((B,) + tuple(shp(m)), dtype=torch.int32, device=self.device)
-      setattr(self.data, name, t)
+    want = None if outputs == 'all' else set(outputs) | {'warning'}
+    for f in DATA_FIELDS.values():
+      # the applied forces are allocated by enable_applied_forces(): writing to them before that must fail loudly, not be ignored
+      if f.role == STATE or (f.role == OUTPUT and (want is None or f.name in want)):
+        self._alloc(f)
     self._bind_io()
-    self._warn_seen = torch.zeros((B, 8), dtype=torch.int32, device=self.device)
+    self._warn_seen = torch.zeros((self.batch, 8), dtype=torch.int32, device=self.device)
     self.reset()
 
   @property
@@ -157,13 +193,20 @@ class BatchedPhysics:
     self._model_flags_version = self.model._flags_version
     self._apply_variable_geoms()       # a re-uploaded model forgets its per-environment geom list
 
+  def _alloc(self, f):
+    setattr(self.data, f.name, torch.zeros((self.batch,) + f.shape(self.model), dtype=f.dtype, device=self.device))
+
   def _bind_io(self):
     for name, ctype in _lib.IO_FIELDS:
       t = getattr(self.data, name, None)
-      if t is None or t.numel() == 0 or (name in ('qfrc_applied', 'xfrc_applied') and not self._applied_on):
+      if t is None or t.numel() == 0 or (name in APPLIED_FIELDS and not self._applied_on):
         setattr(self._io, name, ctypes.cast(None, ctype))
       else:
         setattr(self._io, name, ctypes.cast(t.data_ptr(), ctype))
+
+  def _state_fields(self):
+    """The fields that carry an environment's state: pickled, copied, and uploaded by every call."""
+    return STATE_FIELDS + (APPLIED_FIELDS if self._applied_on else ())
 
   def enable_applied_forces(self, on=True):
     """Allocate `data.qfrc_applied` [B, nv] / `data.xfrc_applied` [B, nbody, 6] and route them into every step (the
@@ -171,10 +214,9 @@ class BatchedPhysics:
     of the split path — and do not exist until enabled, so a write without this call raises AttributeError)."""
     self._pos_current = False
     self._applied_on = bool(on)
-    m, B = self.model, self.batch
-    for name, shape in (('qfrc_applied', (B, m.nv)), ('xfrc_applied', (B, m.nbody, 6))):
+    for name in APPLIED_FIELDS:
       if on and getattr(self.data, name, None) is None:
-        setattr(self.data, name, torch.zeros(shape, dtype=torch.float64, device=self.device))
+        self._alloc(DATA_FIELDS[name])
     self._bind_io()
 
   def free(self):
@@ -206,15 +248,13 @@ class BatchedPhysics:
 
   # ---- pickling (reference: engine.py:287-304 copy / 370-378 __getstate__: model + data travel, the handle is rebuilt) ----
   def __getstate__(self):
-    state = {n: getattr(self.data, n).cpu() for n in ('qpos', 'qvel', 'act', 'qacc_warmstart', 'time', 'ctrl')}
-    if self._applied_on:
-      state['qfrc_applied'] = self.data.qfrc_applied.cpu(); state['xfrc_applied'] = self.data.xfrc_applied.cpu()
+    state = {n: getattr(self.data, n).cpu() for n in self._state_fields()}
     var = getattr(self, '_var_geom_ids', None)
     if var is not None:
       state['var_geom_pos'] = self.data.var_geom_pos.cpu(); state['var_geom_size'] = self.data.var_geom_size.cpu()
     return dict(model=self.model, batch=self.batch, device=str(self.device), sensors=self._sensors, full_final=self._full_final,
                 legacy_step=self.legacy_step, check_errors=self.check_errors, applied=self._applied_on, var_geom_ids=var, state=state,
-                outputs=[n for n, _ in list(self._FIELDS) + list(self._INT_FIELDS) if hasattr(self.data, n)])
+                outputs=[n for n in DATA_FIELDS if hasattr(self.data, n)])
 
   def __setstate__(self, st):
     self.__init__(st['model'], batch=st['batch'], device=st['device'], outputs=st['outputs'], sensors=st['sensors'],
@@ -239,13 +279,12 @@ class BatchedPhysics:
     """A new BatchedPhysics with the same model and a copy of the batched state (reference: engine.py:287-304)."""
     other = type(self)(self.model if share_model else self.model.copy(), batch=self.batch, device=self.device,
                        sensors=self._sensors, full_final=self._full_final)
-    for name in ('qpos', 'qvel', 'act', 'qacc_warmstart', 'time', 'ctrl'):
-      getattr(other.data, name).copy_(getattr(self.data, name))
     other.legacy_step = self.legacy_step
     other.check_errors = self.check_errors
     if self._applied_on:
       other.enable_applied_forces(True)
-      other.data.qfrc_applied.copy_(self.data.qfrc_applied); other.data.xfrc_applied.copy_(self.data.xfrc_applied)
+    for name in self._state_fields():
+      getattr(other.data, name).copy_(getattr(self.data, name))
     other.forward()
     return other
 
@@ -333,7 +372,7 @@ class BatchedPhysics:
     self._pos_current = False
     self._sync_model()
     if env_mask is None:
-      for name in ('qfrc_applied', 'xfrc_applied', 'sensordata', 'actuator_force', 'qacc'):
+      for name in APPLIED_FIELDS + ('sensordata', 'actuator_force', 'qacc'):
         t = getattr(d, name, None)
         if t is not None:
           t.zero_()
@@ -342,7 +381,7 @@ class BatchedPhysics:
         self._warn_seen.zero_()
     else:
       mask = torch.as_tensor(env_mask, dtype=torch.bool, device=self.device)
-      for name in ('qfrc_applied', 'xfrc_applied'):      # mj_resetData clears the applied forces of the reset environments too
+      for name in APPLIED_FIELDS:      # mj_resetData clears the applied forces of the reset environments too
         t = getattr(d, name, None)
         if t is not None:
           t[mask] = 0

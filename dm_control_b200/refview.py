@@ -3,8 +3,8 @@
 `rl/control.py:Environment` can drive this engine: `physics.data.qpos[7:]`, `physics.named.data.xmat['torso', 'zz']`,
 `physics.named.data.qpos[joint_name] = x`, `physics.data.ncon`, `physics.data.contact[i].geom1`, `reset_context()`, ...
 
-The host arrays under `.data` are the state between engine calls: every call uploads qpos / qvel / act / ctrl / time /
-qacc_warmstart / applied forces from them, runs on the device, and downloads state and outputs back IN PLACE (views
+The host arrays under `.data` are the state between engine calls: every call uploads the state fields and applied forces
+of `physics.DATA_FIELDS` from them, runs on the device, and downloads state and outputs back IN PLACE (views
 handed out earlier stay valid, as with MuJoCo's own arrays). It exists for API conformance and debugging — one
 environment per process is the reference's execution model, not this engine's.
 """
@@ -19,9 +19,7 @@ import torch
 from . import index as _index
 from . import mjcf_compile
 from . import lib as _lib
-from .physics import BatchedPhysics, PhysicsError
-
-_STATE = ('qpos', 'qvel', 'act', 'ctrl', 'time', 'qacc_warmstart', 'qfrc_applied', 'xfrc_applied')
+from .physics import APPLIED_FIELDS, STATE_FIELDS, BatchedPhysics, PhysicsError
 
 
 class _Contact:
@@ -98,17 +96,8 @@ class SingleEnvPhysics:
     self._b.enable_applied_forces(True)
     self.model = _WritableModel(model)
     self.data = _HostData(self._b)
-    arrays = self.data._arrays
-    def data_get(name):
-      if name in ('xpos', 'xipos', 'subtree_com', 'subtree_linvel', 'geom_xpos', 'site_xpos'):
-        return arrays[name].reshape(-1, 3) if name in arrays else None
-      if name in ('xmat', 'geom_xmat', 'site_xmat'):
-        return arrays[name].reshape(-1, 9) if name in arrays else None
-      if name == 'xquat':
-        return arrays[name].reshape(-1, 4) if name in arrays else None
-      return arrays.get(name)
     named_model = _index.NamedIndexStructs(types.SimpleNamespace(model=model, data=types.SimpleNamespace())).model
-    self.named = types.SimpleNamespace(data=_index._Struct(data_get, model, False), model=named_model)
+    self.named = types.SimpleNamespace(data=_index._Struct(self.data._arrays.get, model, False), model=named_model)
     self._pull()
     self._reload_from_data(self.data)
 
@@ -146,7 +135,7 @@ class SingleEnvPhysics:
   # ---- host <-> device ----
   def _push(self):
     a, d = self.data._arrays, self._b.data
-    for name in _STATE:
+    for name in STATE_FIELDS + APPLIED_FIELDS:
       t = getattr(d, name, None)
       if t is not None and name in a and t.numel():
         t[0].copy_(torch.as_tensor(np.ascontiguousarray(a[name]).reshape(tuple(t.shape[1:]))))

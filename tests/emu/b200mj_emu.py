@@ -13,7 +13,7 @@ import subprocess
 import numpy as np
 
 from dm_control_b200 import lib as blib
-from dm_control_b200.physics import BatchedPhysics
+from dm_control_b200.physics import APPLIED_FIELDS, STATE_FIELDS, BatchedPhysics
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(os.path.dirname(_HERE))
@@ -71,12 +71,11 @@ class EmuPhysics:
       setattr(self.data, name, np.zeros((batch,) + tuple(shp(model)), np.float64))
     for name, shp in BatchedPhysics._INT_FIELDS:
       setattr(self.data, name, np.zeros((batch,) + tuple(shp(model)), np.int32))
-    state = ('qpos', 'qvel', 'act', 'qacc_warmstart', 'time', 'ctrl', 'qfrc_applied', 'xfrc_applied', 'warning')
     for name, ctype in blib.IO_FIELDS:
       a = getattr(self.data, name, None)
-      if outputs != 'all' and name not in state and name not in outputs:
+      if outputs != 'all' and name not in STATE_FIELDS + APPLIED_FIELDS + ('warning',) and name not in outputs:
         a = None                                   # this output pointer crosses the ABI as NULL
-      if a is None or a.size == 0 or (name in ('qfrc_applied', 'xfrc_applied') and not applied_forces):
+      if a is None or a.size == 0 or (name in APPLIED_FIELDS and not applied_forces):
         setattr(self._io, name, ctypes.cast(None, ctype))
       else:
         setattr(self._io, name, ctypes.cast(a.ctypes.data, ctype))
