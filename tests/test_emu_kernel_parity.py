@@ -17,6 +17,9 @@ import pytest
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), 'emu'))
 import b200mj_emu as emu   # noqa: E402
 
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import dof_models   # noqa: E402
+
 from dm_control_b200 import testing_models as tm   # noqa: E402
 
 pytestmark = pytest.mark.timeout(600)
@@ -29,8 +32,7 @@ def relerr(a, b):
 
 
 def _setup(name, B, seed, oracle_mod, **kw):
-  model = tm.load(name)
-  q0, v0 = tm.initial_states(model, name, B, seed)
+  model, q0, v0 = dof_models.load(name, B, seed)
   p = emu.EmuPhysics(model, B, **kw)
   p.data.qpos[:] = q0; p.data.qvel[:] = v0
   p.forward()
@@ -59,7 +61,8 @@ def test_forward_fields(name, B, oracle_mod):
 
 
 @pytest.mark.parametrize('name,B,ncontrol,nsub', [('cartpole', 8, 60, 1), ('pendulum_free', 8, 50, 2), ('cheetah', 16, 100, 1),
-                                                   ('humanoid', 16, 20, 5), ('quadruped', 8, 15, 4), ('cmu_humanoid', 4, 6, 6)])
+                                                   ('humanoid', 16, 20, 5), ('quadruped', 8, 15, 4), ('cmu_humanoid', 4, 6, 6)] +
+                         [(dof_models.name(nv), 3, 8, 2) for nv in dof_models.NV_TARGETS])      # tests/dof_models.py
 def test_rollout(name, B, ncontrol, nsub, oracle_mod):
   """Fixed action tape, legacy step ordering (engine.py:147-162); every control step is compared: state to 1e-8,
   contact count and geom pairs exactly, sensors to 1e-7."""

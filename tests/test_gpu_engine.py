@@ -8,6 +8,9 @@ torch = pytest.importorskip('torch')
 from conftest import DEV, EMULATE                   # noqa: E402  ('cuda'; 'cpu' only under B200MJ_EMULATE_GPU=1)
 from dm_control_b200 import testing_models as tm   # noqa: E402
 from dm_control_b200 import mjcf_compile as mc    # noqa: E402
+import os, sys   # noqa: E402
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import dof_models   # noqa: E402
 
 
 def _phys(name, B, **kw):
@@ -207,6 +210,34 @@ def test_fused_and_split_paths_agree_bitwise(monkeypatch):
     assert np.abs(a - b).max() <= 1e-8 * (1 + np.abs(b).max()), (f, np.abs(a - b).max())
 
 
+@pytest.mark.parametrize('nv', [6, 9, 12, 18, 22, 27])
+def test_compile_time_size_kernels_match_runtime_size_path(nv, monkeypatch):
+  """For every nv with a compile-time-size acceleration kernel (B200MJ_NV_LIST), a contact rollout of a generated model
+  agrees to 1e-8 with the runtime-size kernels that B200MJ_TN=0 selects at model creation."""
+  from dm_control_b200.physics import BatchedPhysics
+  import numpy as np
+  B = 13
+  model, q0, v0 = dof_models.load(dof_models.name(nv), B, 0)
+  tape = np.random.RandomState(1).uniform(-1, 1, (12, B, model.nu))
+
+  def run():
+    p = BatchedPhysics(model, batch=B)
+    p.data.qpos.copy_(torch.as_tensor(q0)); p.data.qvel.copy_(torch.as_tensor(v0)); p.forward()
+    ncon = 0
+    for t in range(len(tape)):
+      p.set_control(torch.as_tensor(tape[t])); p.step(2)
+      ncon += int(p.data.ncon.sum())
+    assert int(p.data.warning.sum()) == 0
+    return p.data.qpos.cpu().numpy(), p.data.qvel.cpu().numpy(), ncon
+
+  qa, va, na = run()
+  monkeypatch.setenv('B200MJ_TN', '0')
+  qb, vb, nb = run()
+  assert na == nb and na > 0
+  for a, b in ((qa, qb), (va, vb)):
+    assert np.abs(a - b).max() <= 1e-8 * max(1.0, np.abs(b).max()), (nv, np.abs(a - b).max())
+
+
 SLIDING_CUBE = """
 <mujoco><option gravity="0 0 -9.81"/><worldbody>
   <geom name="floor" type="plane" pos="0 0 0" size="10 10 0.1"/>
@@ -322,6 +353,7 @@ def test_per_environment_geoms(oracle_mod):
     ('condim 6 (rolling friction)', '<mujoco><worldbody><geom type="plane" size="1 1 .1"/><body pos="0 0 .2"><freejoint/><geom size=".1" condim="6"/></body></worldbody></mujoco>'),
     ('CG solver', '<mujoco><option solver="CG"/><worldbody><geom type="plane" size="1 1 .1"/><body pos="0 0 .2"><freejoint/><geom size=".1"/></body></worldbody></mujoco>'),
     ('elliptic cones', '<mujoco><option cone="elliptic"/><worldbody><geom type="plane" size="1 1 .1"/><body pos="0 0 .2"><freejoint/><geom size=".1"/></body></worldbody></mujoco>'),
+    ('nv = 65, one more than the largest supported', dof_models.xml(65)),
 ])
 def test_unsupported_features_are_refused_not_approximated(feature, xml):
   """wrapper/core_test.py:426-462 pins contact torques for condim 4 / 6: this engine has condim 1 / 3 only, and a model

@@ -12,6 +12,10 @@ pytestmark = pytest.mark.gpu
 torch = pytest.importorskip('torch')
 from dm_control_b200 import testing_models as tm   # noqa: E402
 
+import os, sys   # noqa: E402
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import dof_models   # noqa: E402
+
 TOL = 1e-8          # asserted; north_star bar is 1e-5
 FIELD_TOL = 1e-10
 
@@ -23,8 +27,7 @@ def relerr(a, b):
 
 def _setup(name, B, seed, oracle_mod):
   from dm_control_b200.physics import BatchedPhysics
-  model = tm.load(name)
-  q0, v0 = tm.initial_states(model, name, B, seed)
+  model, q0, v0 = dof_models.load(name, B, seed)
   phys = BatchedPhysics(model, batch=B)
   phys.data.qpos.copy_(torch.as_tensor(q0))
   phys.data.qvel.copy_(torch.as_tensor(v0))
@@ -64,7 +67,10 @@ def test_forward_fields_match_oracle(name, B, oracle_mod):
 
 @pytest.mark.parametrize('name,B,ncontrol,nsub', [('cartpole', 16, 60, 1), ('pendulum_free', 8, 50, 2),
                                                    ('cheetah', 32, 100, 1), ('humanoid', 32, 20, 5),
-                                                   ('quadruped', 16, 15, 4), ('cmu_humanoid', 6, 6, 6)])
+                                                   ('quadruped', 16, 15, 4), ('cmu_humanoid', 6, 6, 6)] +
+                         # generated models (tests/dof_models.py) at the dof counts no fixture has: the compile-time-size
+                         # kernels and the runtime-size boundaries; B = 13 leaves the last 4-warp and 5-warp CTAs partly filled
+                         [(dof_models.name(nv), B, 12, 2) for nv in dof_models.NV_TARGETS for B in (8, 13)])
 def test_rollout_matches_oracle(name, B, ncontrol, nsub, oracle_mod):
   """Fixed recorded action tape, legacy step ordering; compare every control step."""
   model, phys, oracles = _setup(name, B, 0, oracle_mod)
