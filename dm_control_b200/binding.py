@@ -5,7 +5,8 @@ The reference binds `mjcf.Element`s; the PyMJCF object model is out of scope her
 `physics.bind('geom', 'wall_3').pos`. What carries over is the contract:
 
   * one attribute namespace per element kind with the type prefix removed (`geom_pos` -> `.pos`, `body_mass` -> `.mass`,
-    `jnt_range` -> `.range`, `actuator_gear` -> `.gear`), data fields by their own name (`xpos`, `qpos`, `qvel`, `ctrl`,
+    `jnt_range` -> `.range`, `actuator_gear` -> `.gear`; a joint's `.damping` / `.armature` are the dof_damping /
+    dof_armature columns of its dofs, ragged like its `qvel`), data fields by their own name (`xpos`, `qpos`, `qvel`, `ctrl`,
     `sensordata`, `subtree_linvel`, ...), `element_id`;
   * ragged fields resolve through the address tables (`qpos`/`qvel` of a joint, `sensordata` of a sensor);
   * writes to the STATE through a binding (the fields `physics.DATA_FIELDS` marks STATE) mark the physics dirty, and the
@@ -24,8 +25,24 @@ from .physics import DATA_FIELDS, STATE
 
 _PREFIX = dict(body='body_', geom='geom_', site='site_', joint='jnt_', actuator='actuator_', sensor='sensor_', tendon='tendon_',
                dof='dof_')
+# model fields a joint reaches through its dofs (mjcf/physics.py binds a joint's `damping` / `armature` to dof_damping /
+# dof_armature the same way): ragged, one column per dof of the bound joints
+_MODEL_ALIAS = {'joint': {'damping': 'dof_damping', 'armature': 'dof_armature'}}
 _DATA_ALIAS = {'geom': {'xpos': 'geom_xpos', 'xmat': 'geom_xmat'}, 'site': {'xpos': 'site_xpos', 'xmat': 'site_xmat'},
                'actuator': {'force': 'actuator_force'}}
+
+
+def model_field(kind, attr):
+  """The model field behind attribute `attr` of a bound `kind` element."""
+  return _MODEL_ALIAS.get(kind, {}).get(attr, _PREFIX[kind] + attr)
+
+
+def model_rows(model, kind, field, ids):
+  """(ragged, rows of `field` that belong to the elements `ids` of `kind`): a joint's dofs for the dof fields."""
+  if field.startswith('dof_') and kind == 'joint':
+    slices = index._ragged(model, 'nv')
+    return True, [c for i in ids for c in range(slices[i].start, slices[i].stop)]
+  return False, [int(i) for i in ids]
 
 
 class Binding:
@@ -61,6 +78,11 @@ class Binding:
     t = getattr(d, name, None)
     return (name, t) if isinstance(t, torch.Tensor) else (name, None)
 
+  def _env_rows(self, mname):
+    """[B, n, w] view of a per-environment model field (physics.set_env_model_fields)."""
+    t = getattr(self._p.env_model, mname)
+    return t.reshape(t.shape[0], t.shape[1], -1)
+
   def _squeeze(self, t):
     return t[:, 0] if self._single and t.dim() >= 2 else t
 
@@ -74,12 +96,20 @@ class Binding:
         p.forward()                              # lazily, once: derived quantities after a state write through a binding
       out = t.index_select(1, idx)
       return out if ragged else self._squeeze(out)
-    mname = _PREFIX[self._kind] + name
+    mname = model_field(self._kind, name)
+    if mname in getattr(p, 'env_model_fields', ()):          # per-environment model field: [B, k(, w)]
+      ragged, rows = model_rows(p.model, self._kind, mname, self._ids)
+      out = self._env_rows(mname)[:, torch.as_tensor(rows, dtype=torch.int64, device=p.device)]
+      out = out[..., 0] if out.shape[2] == 1 else out
+      return out if ragged else self._squeeze(out)
     arr = p.model.fields.get(mname)
     if arr is None:
       raise AttributeError(f'bound {self._kind} has no attribute {name!r}')
+    ragged, idx = model_rows(p.model, self._kind, mname, self._ids)
+    if ragged:
+      return np.asarray(arr)[idx]
     n = len(p.model.ordered_names[self._kind]) if self._kind in p.model.ordered_names else arr.shape[0]
-    rows = np.asarray(arr).reshape(n, -1)[self._ids]
+    rows = np.asarray(arr).reshape(n, -1)[idx]
     rows = rows[:, 0] if rows.shape[1] == 1 else rows
     return rows[0] if self._single else rows
 
@@ -100,10 +130,30 @@ class Binding:
         if field != 'ctrl':                      # ctrl does not invalidate position / velocity-stage quantities
           object.__setattr__(p, '_bind_dirty', True)
       return
-    mname = _PREFIX[self._kind] + name
+    mname = model_field(self._kind, name)
+    if mname in getattr(p, 'env_model_fields', ()):          # per-environment model field: [B, k, w], [k, w] or a scalar
+      rows = self._env_rows(mname)
+      _, idx = model_rows(p.model, self._kind, mname, self._ids)
+      tidx = torch.as_tensor(idx, dtype=torch.int64, device=p.device)
+      k, w = len(idx), rows.shape[2]
+      v = torch.as_tensor(value, dtype=rows.dtype, device=p.device)
+      n = v.numel()
+      shape = (p.batch, k, w) if n == p.batch * k * w and n != k * w else (1, k, w) if n == k * w else (1, 1, w) if n == w else (1, 1, 1)
+      if n != shape[0] * shape[1] * shape[2]:
+        raise ValueError(f'{name!r}: cannot write a value of shape {tuple(v.shape)} to [{p.batch}, {k}, {w}]')
+      rows[:, tidx] = v.reshape(shape).expand(p.batch, k, w)
+      p.mark_as_dirty()
+      object.__setattr__(p, '_bind_dirty', True)
+      return
     if mname not in p.model.fields:
       raise AttributeError(f'bound {self._kind} has no attribute {name!r}')
     arr = p.model.fields[mname]
+    ragged, idx = model_rows(p.model, self._kind, mname, self._ids)
+    if ragged:
+      arr[idx] = np.asarray(value, dtype=arr.dtype)
+      p.model.touch()
+      object.__setattr__(p, '_bind_dirty', True)
+      return
     n = len(p.model.ordered_names[self._kind])
     arr.reshape(n, -1)[self._ids] = np.asarray(value, dtype=arr.dtype).reshape(len(self._ids), -1) if np.ndim(value) else value
     p.model.touch()

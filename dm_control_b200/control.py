@@ -60,6 +60,7 @@ class BatchedEnvironment:
     # buffer; returned tensors are static buffers that the next step overwrites.
     self._graph_step = graph_step
     self._step_graphs = {}
+    self._graph_epoch = None          # the physics' _launch_epoch the graphs were captured at
     # Optional device-side epilogue of a control step, `hook(reward, observation, discount)`: runs (and is captured)
     # with the step — e.g. packing the observation dict into one [B, k] block for a single device->host copy.
     self.post_step_hook = None
@@ -137,6 +138,11 @@ class BatchedEnvironment:
 
   def _graphed_step(self, action):
     phys = self._physics
+    phys._sync_model()
+    if self._graph_epoch != phys._launch_epoch:
+      # a captured step launches with the model, io and per-environment tables of its capture: re-capture after any change
+      self._step_graphs.clear()
+      self._graph_epoch = phys._launch_epoch
     key = phys._flags()
     entry = self._step_graphs.get(key)
     if entry is None:

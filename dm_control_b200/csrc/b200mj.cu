@@ -41,6 +41,14 @@
 // ------------------------------------------------------------------------------------------------
 // device model view + workspace layout
 // ------------------------------------------------------------------------------------------------
+// The model fields an environment may hold values of its own (b200mj_model_set_env_fields). Only tables that nothing
+// derived at model creation depends on, and that change no launch-wide choice (culls, row counts, kernel builds).
+#define ENV_FIELDS(X) X(body_mass) X(body_inertia) X(body_ipos) X(geom_friction) X(geom_solref) X(geom_solimp) \
+  X(dof_damping) X(dof_armature) X(jnt_stiffness) X(actuator_gainprm) X(actuator_biasprm)
+#define ENV_ENUM(name) EF_##name,
+enum { ENV_FIELDS(ENV_ENUM) ENV_NFIELDS };
+#undef ENV_ENUM
+
 struct DevModel {
 #define DECL_I(name) const int* name;
 #define DECL_R(name) const double* name;
@@ -59,6 +67,11 @@ struct DevModel {
   int cvx_warp;     // convex pairs resolved by the whole warp (cvx_pair_warp; B200MJ_CVX_WARP=0: one pair per lane, cvx_pair)
   double timestep, gravity[3], tolerance, ls_tolerance, impratio, meaninertia;
 };
+
+// Per-environment model fields (b200mj_model_set_env_fields): field f of ENV_FIELDS is read from
+// rows + env * row + off[f] where off[f] >= 0, else from the shared DevModel table. A kernel parameter of its own, so
+// that DevModel and Ctx, and with them the code of the builds without per-environment fields, stay as they were.
+struct EnvModel { const double* rows; int row; int off[ENV_NFIELDS]; };
 
 // offsets (in doubles) into one environment's workspace
 struct Lay {
@@ -126,6 +139,9 @@ struct b200mj_model {
   double* d_rdata;
   int* d_xi; double* d_xr;      // derived tables (dof_act_*)
   int* d_varid;                 // geom -> variable-geom slot
+  int env_len[ENV_NFIELDS];     // full length of each per-environment-capable field (doubles)
+  EnvModel em;                  // per-environment model fields (em.rows == nullptr: none)
+  int env_nrows;                // rows behind em.rows (0: none); calls may cover at most that many environments
   int envs_per_block;
   size_t smem_per_env;
   int tn_nv;                  // nv when a compile-time-size acceleration kernel exists for this model, else 0
@@ -258,13 +274,25 @@ struct Ctx {
   const double* Jg;     // acceleration stage: this environment's constraint Jacobian in the handover row (L.jalias)
   const double* Mc;     // acceleration stage: the joint-space inertia, read-only — the workspace copy, or (L.mglobal) the handover row in L2
   int env; const double* var_pos; const double* var_size;      // per-environment geoms (set_env)
-  __device__ void set_env(int e, const b200mj_io& io) { env = e; var_pos = io.var_geom_pos; var_size = io.var_geom_size; }
-  __device__ Ctx(const DevModel& m_, const Lay& L_, double* ws_, int lane_, int df, int ns) : m(m_), L(L_), ws(ws_), lane(lane_), disableflags(df), newton_sync(ns), env(0), var_pos(nullptr), var_size(nullptr) {
+  const EnvModel* em;   // per-environment model fields: the kernel's EnvModel in the ENVM builds, nullptr in the others (MF)
+  __device__ void set_env(int e, const b200mj_io& io, const EnvModel* em_) { env = e; var_pos = io.var_geom_pos; var_size = io.var_geom_size; em = em_; }
+  __device__ Ctx(const DevModel& m_, const Lay& L_, double* ws_, int lane_, int df, int ns) : m(m_), L(L_), ws(ws_), lane(lane_), disableflags(df), newton_sync(ns), env(0), var_pos(nullptr), var_size(nullptr), em(nullptr) {
     pM = ws_ + L_.M; pJ = ws_ + L_.J; pD = ws_ + L_.efcD; pAref = ws_ + L_.aref; pBias = ws_ + L_.bias; pPassive = ws_ + L_.passive;
     pEq = reinterpret_cast<int*>(ws_ + L_.eqflag); stage = ws_ + L_.J; Mc = pM; Jg = pJ;
   }
 };
 #define W(name) (c.ws + c.L.name)
+
+// field f's table as environment `env` sees it: its row of the per-environment fields, or the shared model's.
+// Resolved where the field is read, so that no pointer stays live across the stages in between.
+__device__ __forceinline__ const double* env_table(const EnvModel& em, int env, int f, const double* shared) {
+  const int o = em.off[f];
+  return o < 0 ? shared : em.rows + (size_t)env * em.row + o;
+}
+// The same inside the stage functions. c.em is a compile-time constant once the stages are inlined (nullptr in the builds
+// without per-environment fields, which then read the shared tables exactly as before: resolving the row at the read
+// sites costs the register-bound kernels spill bytes).
+#define MF(c, f) ((c).em ? env_table(*(c).em, (c).env, EF_##f, (c).m.f) : (c).m.f)
 
 // ------------------------------------------------------------------------------------------------
 // dense Cholesky in the workspace: A (n x n, row stride ld) -> lower factor Lm, same stride
@@ -883,7 +911,8 @@ __device__ __forceinline__ void kinematics(const Ctx& c) {
   }
   // inertial frames' origins and geom frames
   FOR_LANES(b, m.nbody) {
-    double tmp[3], ip[3] = {m.body_ipos[3*b], m.body_ipos[3*b+1], m.body_ipos[3*b+2]};
+    const double* bi = MF(c, body_ipos) + 3 * b;
+    double tmp[3], ip[3] = {bi[0], bi[1], bi[2]};
     mat_vec(tmp, xmat + 9 * b, ip);
     for (int i = 0; i < 3; i++) W(xipos)[3 * b + i] = xpos[3 * b + i] + tmp[i];
   }
@@ -926,7 +955,8 @@ __device__ __forceinline__ void geom_frame(const Ctx& c, int g, double* pos, dou
 __device__ __forceinline__ void com_pos(const Ctx& c) {
   const DevModel& m = c.m; int lane = c.lane;
   double* sc = W(scom); double* xipos = W(xipos);
-  FOR_LANES(b, m.nbody) { double ms = m.body_mass[b]; for (int i = 0; i < 3; i++) sc[3 * b + i] = ms * xipos[3 * b + i]; }
+  const double* body_mass = MF(c, body_mass);
+  FOR_LANES(b, m.nbody) { double ms = body_mass[b]; for (int i = 0; i < 3; i++) sc[3 * b + i] = ms * xipos[3 * b + i]; }
   __syncwarp();
   tree_accumulate(c, sc, 3, true);
   FOR_LANES(b, m.nbody) {
@@ -944,7 +974,8 @@ __device__ __forceinline__ void com_pos(const Ctx& c) {
     int root = m.body_rootid[b];
     double dif[3];
     for (int i = 0; i < 3; i++) dif[i] = xipos[3 * b + i] - sc[3 * root + i];
-    double mass = m.body_mass[b], in0 = m.body_inertia[3*b], in1 = m.body_inertia[3*b+1], in2 = m.body_inertia[3*b+2];
+    const double* bin = MF(c, body_inertia) + 3 * b;
+    double mass = body_mass[b], in0 = bin[0], in1 = bin[1], in2 = bin[2];
     double t[9];
     for (int r = 0; r < 3; r++) for (int cc = 0; cc < 3; cc++)
       t[3 * r + cc] = mat[3 * r] * in0 * mat[3 * cc] + mat[3 * r + 1] * in1 * mat[3 * cc + 1] + mat[3 * r + 2] * in2 * mat[3 * cc + 2];
@@ -1010,7 +1041,7 @@ __device__ __forceinline__ void crb_and_factor(const Ctx& c) {
       const double* cj = W(cdof) + 6 * j;
       double s = 0;
       for (int k = 0; k < 6; k++) s += cj[k] * buf[k];
-      if (j == i) s += m.dof_armature[i];
+      if (j == i) s += MF(c, dof_armature)[i];
       M[tri(i) + j] = s;      // packed lower triangle: j walks the ancestors of i, so j <= i
     }
   }
@@ -1509,9 +1540,9 @@ __device__ __forceinline__ int collision(const Ctx& c, int* warn_contactfull) {
       for (int i = 0; i < 3; i++) { rec[1 + i] = STG(k, 1 + i); nrm[i] = STG(k, 4 + i); tan[i] = STG_TAN(i); }
       make_frame(rec + 4, nrm, tan);
       int pr1 = m.geom_priority[g1], pr2 = m.geom_priority[g2];
-      int condim; double mu;
-      if (pr1 != pr2) { int gp = pr1 > pr2 ? g1 : g2; condim = m.geom_condim[gp]; mu = m.geom_friction[3 * gp]; }
-      else { condim = max(m.geom_condim[g1], m.geom_condim[g2]); mu = fmax(m.geom_friction[3 * g1], m.geom_friction[3 * g2]); }
+      int condim; double mu; const double* fr = MF(c, geom_friction);
+      if (pr1 != pr2) { int gp = pr1 > pr2 ? g1 : g2; condim = m.geom_condim[gp]; mu = fr[3 * gp]; }
+      else { condim = max(m.geom_condim[g1], m.geom_condim[g2]); mu = fmax(fr[3 * g1], fr[3 * g2]); }
       rec[13] = mu;
       int* ii = con_ints(rec);
       ii[0] = g1; ii[1] = g2; ii[2] = condim; ii[3] = -1;
@@ -1681,21 +1712,22 @@ __device__ __forceinline__ int make_constraint(const Ctx& c, int ncon, int* warn
     double vn = warp_sum(pv[0]);
     // contact parameter mixing (solref / solimp)
     double solref[2], solimp[5];
+    const double* geom_solref = MF(c, geom_solref); const double* geom_solimp = MF(c, geom_solimp);
     int pr1 = m.geom_priority[g1], pr2 = m.geom_priority[g2];
     if (pr1 != pr2) {
       int gp = pr1 > pr2 ? g1 : g2;
-      for (int i = 0; i < 2; i++) solref[i] = m.geom_solref[2 * gp + i];
-      for (int i = 0; i < 5; i++) solimp[i] = m.geom_solimp[5 * gp + i];
+      for (int i = 0; i < 2; i++) solref[i] = geom_solref[2 * gp + i];
+      for (int i = 0; i < 5; i++) solimp[i] = geom_solimp[5 * gp + i];
     } else {
       double s1 = m.geom_solmix[g1], s2 = m.geom_solmix[g2], mix;
       if (s1 >= BMJ_MINVAL && s2 >= BMJ_MINVAL) mix = s1 / (s1 + s2);
       else if (s1 < BMJ_MINVAL && s2 < BMJ_MINVAL) mix = 0.5;
       else if (s1 < BMJ_MINVAL) mix = 0.0; else mix = 1.0;
-      if (m.geom_solref[2 * g1] > 0 && m.geom_solref[2 * g2] > 0)
-        for (int i = 0; i < 2; i++) solref[i] = mix * m.geom_solref[2 * g1 + i] + (1 - mix) * m.geom_solref[2 * g2 + i];
+      if (geom_solref[2 * g1] > 0 && geom_solref[2 * g2] > 0)
+        for (int i = 0; i < 2; i++) solref[i] = mix * geom_solref[2 * g1 + i] + (1 - mix) * geom_solref[2 * g2 + i];
       else
-        for (int i = 0; i < 2; i++) solref[i] = fmin(m.geom_solref[2 * g1 + i], m.geom_solref[2 * g2 + i]);
-      for (int i = 0; i < 5; i++) solimp[i] = mix * m.geom_solimp[5 * g1 + i] + (1 - mix) * m.geom_solimp[5 * g2 + i];
+        for (int i = 0; i < 2; i++) solref[i] = fmin(geom_solref[2 * g1 + i], geom_solref[2 * g2 + i]);
+      for (int i = 0; i < 5; i++) solimp[i] = mix * geom_solimp[5 * g1 + i] + (1 - mix) * geom_solimp[5 * g2 + i];
     }
     double tran = m.body_invweight0[2 * b1] + m.body_invweight0[2 * b2];
     if (dim == 1) {
@@ -1780,11 +1812,12 @@ __device__ __forceinline__ void fwd_velocity(const Ctx& c) {
     double ps = 0;
     if (!(c.disableflags & BMJ_DSBL_PASSIVE)) {
       int j = m.dof_jntid[k], t = m.jnt_type[j];
-      if ((t == BMJ_JNT_SLIDE || t == BMJ_JNT_HINGE) && m.jnt_stiffness[j] != 0) {
+      const double stiff = MF(c, jnt_stiffness)[j];
+      if ((t == BMJ_JNT_SLIDE || t == BMJ_JNT_HINGE) && stiff != 0) {
         int qa = m.jnt_qposadr[j];
-        ps -= m.jnt_stiffness[j] * (W(qpos)[qa] - m.qpos_spring[qa]);
+        ps -= stiff * (W(qpos)[qa] - m.qpos_spring[qa]);
       }
-      ps -= m.dof_damping[k] * qvel[k];
+      ps -= MF(c, dof_damping)[k] * qvel[k];
     }
     c.pPassive[k] = ps;
   }
@@ -1799,7 +1832,8 @@ __device__ __forceinline__ void subtree_vel(const Ctx& c) {
     double dif[3], tmp[3];
     for (int i = 0; i < 3; i++) dif[i] = W(xipos)[3 * b + i] - W(scom)[3 * root + i];
     cross3(tmp, dif, W(cvel) + 6 * b);
-    for (int i = 0; i < 3; i++) sl[3 * b + i] = m.body_mass[b] * (W(cvel)[6 * b + 3 + i] - tmp[i]);
+    const double mass = MF(c, body_mass)[b];
+    for (int i = 0; i < 3; i++) sl[3 * b + i] = mass * (W(cvel)[6 * b + 3 + i] - tmp[i]);
   }
   __syncwarp();
   tree_accumulate(c, sl, 3, true);
@@ -1835,7 +1869,7 @@ __device__ __forceinline__ void fwd_actuation(const Ctx& c) {
         double s = 0; _Pragma("unroll 1") for (int i = 0; i < nv; i++) s += gear * W(tenJ)[t * ld + i] * W(qvel)[i];
         velocity = s;
       }
-      const double* gp = m.actuator_gainprm + 3 * a; const double* bp = m.actuator_biasprm + 3 * a;
+      const double* gp = MF(c, actuator_gainprm) + 3 * a; const double* bp = MF(c, actuator_biasprm) + 3 * a;
       double gain = gp[0];
       if (m.actuator_gaintype[a] == BMJ_GAIN_AFFINE) gain += gp[1] * length + gp[2] * velocity;
       double bias = 0;
@@ -2505,24 +2539,38 @@ __device__ __forceinline__ void reset_state(const Ctx& c, double* time) {
   __syncwarp();
 }
 
+// mj_Euler's choice of the implicit damping update, made per environment: some entry of its dof_damping is positive
+// (the model's flag, or a warp vote over the environment's own row; the rows may change between graph replays).
+// DAMPED: the builds without per-environment fields test the model's flag exactly where they did before. (Read sites
+// stay inside their loops too: a table pointer hoisted out of the Euler loops cost the 27-dof kernel 4 bytes of spills.)
+#define DAMPED(c) ((c).em ? env_damped(c) : (c).m.any_damping)
+__device__ __forceinline__ bool env_damped(const Ctx& c) {
+  const DevModel& m = c.m; int lane = c.lane;
+  if (c.em->off[EF_dof_damping] < 0) return m.any_damping;
+  const double* d = MF(c, dof_damping);
+  int any = 0;
+  FOR_LANES(i, m.nv) if (d[i] > 0) any = 1;
+  return __any_sync(FULL, any);
+}
+
 template <int NVT>
 __device__ __forceinline__ void euler_step(const Ctx& c, double* time) {
   const DevModel& m = c.m; int lane = c.lane; int nv = m.nv, ld = m.ldv; double h = m.timestep;
   advance_act(c, W(act), W(actdot), 1.0, h);
-  if (NVT > 0 && m.any_damping && !(c.disableflags & BMJ_DSBL_EULERDAMP)) {
+  if (NVT > 0 && DAMPED(c) && !(c.disableflags & BMJ_DSBL_EULERDAMP)) {
     if constexpr (NVT > 0) {
       // M is dead after the solver: M + h diag(damping) is formed in place
-      FOR_LANES(i, nv) { W(tmpv)[i] = W(smooth)[i] + W(qcon)[i]; W(M)[tri(i) + i] += h * m.dof_damping[i]; }
+      FOR_LANES(i, nv) { W(tmpv)[i] = W(smooth)[i] + W(qcon)[i]; W(M)[tri(i) + i] += h * MF(c, dof_damping)[i]; }
       __syncwarp();
       tn_factor<NVT>(W(M), W(H), W(dinv), lane, W(tmpv), W(tmpv), W(J), W(efcSD), reinterpret_cast<const int*>(W(actlist)), opaque_zero(), W(colbuf));
       tn_back<NVT>(W(H), W(dinv), W(tmpv), W(tmpv), lane, 0);
       FOR_LANES(i, nv) W(qvel)[i] += h * W(tmpv)[i];
     }
-  } else if (m.any_damping && !(c.disableflags & BMJ_DSBL_EULERDAMP)) {
+  } else if (DAMPED(c) && !(c.disableflags & BMJ_DSBL_EULERDAMP)) {
     copy_row(W(H), c.Mc, tri(nv), lane);
     FOR_LANES(i, nv) W(tmpv)[i] = W(smooth)[i] + W(qcon)[i];
     __syncwarp();
-    FOR_LANES(i, nv) W(H)[tri(i) + i] += h * m.dof_damping[i];
+    FOR_LANES(i, nv) W(H)[tri(i) + i] += h * MF(c, dof_damping)[i];
     __syncwarp();
     chol_factor(W(H), W(H), W(dinv), nv, lane, W(tmpv), W(tmpv));
     chol_back(W(H), W(dinv), W(tmpv), W(tmpv), nv, lane);
@@ -2605,10 +2653,11 @@ enum { MODE_STEP = 0, MODE_FORWARD = 1 };
 //   pass kinds: [posvel + acc + integrate] x nstep  (RK4: 4 passes per step), then for the reference's legacy
 //   ordering one trailing [posvel] pass (= mj_step1 on the new state); MODE_FORWARD = one [posvel + acc] pass.
 // CVX: as for the position kernels (the primitive-only build shares narrowphase<false> with them, so the two paths stay bit-identical).
-template <bool CVX>
+// ENVM (here and in the split kernels): the model has per-environment fields (b200mj_model_set_env_fields; MF).
+template <bool CVX, bool ENVM>
 __global__ void __launch_bounds__(256)
 step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ b200mj_io io,
-            int batch, int nstep, int flags, int mode, int extra_disable, const uint8_t* env_mask) {
+            int batch, int nstep, int flags, int mode, int extra_disable, const uint8_t* env_mask, const __grid_constant__ EnvModel em) {
   B200MJ_DYN_SMEM
   int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int env = blockIdx.x * (blockDim.x >> 5) + warp;
@@ -2617,7 +2666,7 @@ step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, c
   const bool live = env < batch && (env_mask == nullptr || env_mask[env < batch ? env : 0] != 0);
   if (env >= batch) env = batch - 1;
   Ctx c(m, L, smem + (size_t)warp * L.total, lane, m.disableflags | extra_disable, 0);
-  c.set_env(env, io);
+  c.set_env(env, io, ENVM ? &em : nullptr);
   size_t e = (size_t)env;
   // ---- load state ----
   FOR_LANES(i, m.nq) W(qpos)[i] = io.qpos[e * m.nq + i];
@@ -2733,10 +2782,11 @@ step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, c
 //   POS_BIG (224, 1): large models (CMU corridor: 30 KB of position workspace per environment, one CTA per SM either
 //     way): up to seven phase-aligned warps in that one CTA and the full register budget
 enum { POS_PRIM, POS_CVX, POS_BIG };
-template <bool FINAL, int BUILD>
+template <bool FINAL, int BUILD, bool ENVM>
 __global__ void __launch_bounds__(BUILD == POS_BIG ? 224 : 160, BUILD == POS_PRIM ? 3 : BUILD == POS_CVX ? 2 : 1)
 pos_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Handover ho,
-           const __grid_constant__ b200mj_io io, int batch, int flags, int dump, int env0, const __grid_constant__ Compact cp) {
+           const __grid_constant__ b200mj_io io, int batch, int flags, int dump, int env0, const __grid_constant__ Compact cp,
+           const __grid_constant__ EnvModel em) {
   constexpr bool CVX = BUILD != POS_PRIM;
   B200MJ_DYN_SMEM
   int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -2748,7 +2798,7 @@ pos_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, co
   const bool live = env < batch;
   if (!live) env = batch - 1;
   Ctx c(m, L, smem + (size_t)warp * L.total, lane, m.disableflags, 0);
-  c.set_env(env, io);
+  c.set_env(env, io, ENVM ? &em : nullptr);
   size_t e = (size_t)env;
   // A shadow warp gets a handover row of its own: the stages read back what they wrote there (raw-contact staging, Jacobian rows), so
   // sharing the live environment's row would race; the io arrays are only ever overwritten with identical values.
@@ -2835,10 +2885,11 @@ pos_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, co
 // quadruped 22, humanoid 27) and a few common small sizes — built for at most 4 warps per CTA. Same arguments, same
 // handover format.
 #define B200MJ_NV_LIST(X) X(6) X(9) X(12) X(18) X(22) X(27)
-template <bool LAST, int NVT>
+template <bool LAST, int NVT, bool ENVM>
 __global__ void __launch_bounds__(NVT > 0 ? 128 : 256, NVT > 0 ? 4 : 0)
 acc_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, const __grid_constant__ Handover ho,
-           const __grid_constant__ b200mj_io io, int first_pass, int flags, const int* bucket_count, const int* bucket_list) {
+           const __grid_constant__ b200mj_io io, int first_pass, int flags, const int* bucket_count, const int* bucket_list,
+           const __grid_constant__ EnvModel em) {
   B200MJ_DYN_SMEM
   int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // One launch per row-count bucket: the CTAs walk the bucket's environment list (*bucket_count entries), which the
@@ -2860,7 +2911,7 @@ acc_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, co
   const int* cnt = reinterpret_cast<const int*>(hrow + H.counts);
   const int ncon = cnt[0], nefc = cnt[1];
   Ctx c(m, L, smem + (size_t)warp * L.total, lane, m.disableflags, sync);
-  c.set_env(env, io);
+  c.set_env(env, io, ENVM ? &em : nullptr);
   const int nv = NVT > 0 ? NVT : m.nv, ld = NVT > 0 ? (NVT | 1) : m.ldv;
   // ---- load state + handover ----
   FOR_LANES(i, m.nq) W(qpos)[i] = io.qpos[e * m.nq + i];
@@ -2918,24 +2969,34 @@ acc_kernel(const __grid_constant__ DevModel m, const __grid_constant__ Lay L, co
 // ------------------------------------------------------------------------------------------------
 static int64_t g_launches = 0;
 
-typedef decltype(&step_kernel<true>) step_kernel_fn;
-typedef decltype(&pos_kernel<false, POS_CVX>) pos_kernel_fn;
-typedef decltype(&acc_kernel<false, 0>) acc_kernel_fn;
+typedef decltype(&step_kernel<true, false>) step_kernel_fn;
+typedef decltype(&pos_kernel<false, POS_CVX, false>) pos_kernel_fn;
+typedef decltype(&acc_kernel<false, 0, false>) acc_kernel_fn;
 
-static step_kernel_fn step_kernel_for(const b200mj_model* M) { return M->convex_pairs ? step_kernel<true> : step_kernel<false>; }
+// every selector picks the ENVM build when the model has per-environment fields
+static bool envm(const b200mj_model* M) { return M->em.rows != nullptr; }
+
+static step_kernel_fn step_kernel_for(const b200mj_model* M) {
+  if (envm(M)) return M->convex_pairs ? step_kernel<true, true> : step_kernel<false, true>;
+  return M->convex_pairs ? step_kernel<true, false> : step_kernel<false, false>;
+}
 
 // final: the trailing mj_step1
+template <bool ENVM> static pos_kernel_fn pos_kernel_build(const b200mj_model* M, bool final) {
+  if (M->pos_big) return final ? pos_kernel<true, POS_BIG, ENVM> : pos_kernel<false, POS_BIG, ENVM>;
+  if (M->convex_pairs) return final ? pos_kernel<true, POS_CVX, ENVM> : pos_kernel<false, POS_CVX, ENVM>;
+  return final ? pos_kernel<true, POS_PRIM, ENVM> : pos_kernel<false, POS_PRIM, ENVM>;
+}
 static pos_kernel_fn pos_kernel_for(const b200mj_model* M, bool final) {
-  if (M->pos_big) return final ? pos_kernel<true, POS_BIG> : pos_kernel<false, POS_BIG>;
-  if (M->convex_pairs) return final ? pos_kernel<true, POS_CVX> : pos_kernel<false, POS_CVX>;
-  return final ? pos_kernel<true, POS_PRIM> : pos_kernel<false, POS_PRIM>;
+  return envm(M) ? pos_kernel_build<true>(M, final) : pos_kernel_build<false>(M, final);
 }
 
 // the acceleration kernel for a compile-time size of nvt dofs (0: the runtime-size kernel), or nullptr where
 // B200MJ_NV_LIST has no kernel for nvt
-static acc_kernel_fn acc_kernel_for(int nvt, bool last) {
+static acc_kernel_fn acc_kernel_for(int nvt, bool last, bool env = false) {
   switch (nvt) {
-#define NV_CASE(n) case n: return last ? acc_kernel<true, n> : acc_kernel<false, n>;
+#define NV_CASE(n) case n: return env ? (last ? acc_kernel<true, n, true> : acc_kernel<false, n, true>) \
+                                      : (last ? acc_kernel<true, n, false> : acc_kernel<false, n, false>);
     NV_CASE(0) B200MJ_NV_LIST(NV_CASE)
 #undef NV_CASE
     default: return nullptr;
@@ -2946,7 +3007,7 @@ static acc_kernel_fn acc_kernel_for(int nvt, bool last) {
 // whenever the layout is rebuilt: a change of capacities can move the model to another position-kernel build.
 static void allow_shared_memory(const b200mj_model* M) {
   const void* kernels[] = {(const void*)step_kernel_for(M), (const void*)pos_kernel_for(M, false), (const void*)pos_kernel_for(M, true),
-                           (const void*)acc_kernel_for(M->tn_nv, false), (const void*)acc_kernel_for(M->tn_nv, true)};
+                           (const void*)acc_kernel_for(M->tn_nv, false, envm(M)), (const void*)acc_kernel_for(M->tn_nv, true, envm(M))};
   for (const void* k : kernels) cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_MAX);
 }
 
@@ -3158,9 +3219,23 @@ struct HostModel {
 #undef HOST_I
 #undef HOST_R
 };
-#define COUNT_FIELD(name) + 1
-static const int NFIELDS = 0 B200MJ_MODEL_FIELDS(COUNT_FIELD, COUNT_FIELD);
-#undef COUNT_FIELD
+// field ids: positions in B200MJ_MODEL_FIELDS
+#define FIELD_ID(name) FID_##name,
+enum { B200MJ_MODEL_FIELDS(FIELD_ID, FIELD_ID) NFIELDS };
+#undef FIELD_ID
+
+// the ENV_FIELDS index of model field `fid`, or -1 where the field cannot vary per environment
+static int env_field_of(int fid) {
+  switch (fid) {
+#define ENV_CASE(name) case FID_##name: return EF_##name;
+    ENV_FIELDS(ENV_CASE)
+#undef ENV_CASE
+    default: return -1;
+  }
+}
+
+// the per-environment model fields, when set, must have a row for every environment a call covers
+static bool env_rows_cover(const b200mj_model* M, int batch) { return M->env_nrows == 0 || batch <= M->env_nrows; }
 
 extern "C" {
 
@@ -3174,6 +3249,12 @@ const char* b200mj_error_string(int code) {
     case -3: return "model feature outside the supported subset (condim 4/6, frictionloss, nv > 64, CG solver, elliptic cones, mesh / hfield geoms)";
     case -4: return "per-environment workspace exceeds 227 KB of shared memory: lower nconmax / njmax";
     case -5: return "kernel launch failed";
+    case -6: return "model field cannot vary per environment (supported: body_mass, body_inertia, body_ipos, geom_friction, "
+                    "geom_solref, geom_solimp, dof_damping, dof_armature, jnt_stiffness, actuator_gainprm, actuator_biasprm)";
+    case -7: return "model field listed twice for per-environment values";
+    case -8: return "per-environment model fields without rows (rows_dev is NULL)";
+    case -9: return "per-environment model fields need at least one row (nrows < 1)";
+    case -10: return "batch exceeds the rows of the per-environment model fields";
     default: return "unknown error";
   }
 }
@@ -3237,6 +3318,9 @@ int b200mj_model_create(const int32_t* idata, int ni, const double* rdata, int n
   m.impratio = optr[BMJ_OPT_IMPRATIO]; m.meaninertia = optr[BMJ_OPT_MEANINERTIA];
   m.any_damping = 0;
   for (int i = 0; i < m.nv; i++) if (h.dof_damping.p[i] > 0) m.any_damping = 1;
+#define ENV_LEN(name) M->env_len[EF_##name] = h.name.n; M->em.off[EF_##name] = -1;
+  ENV_FIELDS(ENV_LEN)
+#undef ENV_LEN
   m.acc_sensors = 0;
   for (int i = 0; i < h.sensor_type.n; i++) { int t = h.sensor_type.p[i]; if (t == BMJ_SENS_ACCELEROMETER || t == BMJ_SENS_FORCE || t == BMJ_SENS_TORQUE) m.acc_sensors = 1; }
   bool unsupported = m.nv > 64 || (opti[BMJ_OPT_SOLVER] != BMJ_SOL_NEWTON && opti[BMJ_OPT_SOLVER] != BMJ_SOL_PGS) || opti[BMJ_OPT_CONE] != 0 ||
@@ -3366,7 +3450,7 @@ extern "C" __global__ void b200mj_reset_kernel(const __grid_constant__ DevModel 
 
 // mj_contactForce for one contact id of every environment (one thread per environment)
 extern "C" __global__ void b200mj_contact_force_kernel(const __grid_constant__ DevModel m, const __grid_constant__ b200mj_io io,
-                                                       int batch, int cid, double* out6) {
+                                                       int batch, int cid, double* out6, const __grid_constant__ EnvModel em) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= batch) return;
   double f[6] = {0, 0, 0, 0, 0, 0};
@@ -3377,9 +3461,10 @@ extern "C" __global__ void b200mj_contact_force_kernel(const __grid_constant__ D
     if (adr >= 0) {
       const int g1 = io.contact_geom[2 * o], g2 = io.contact_geom[2 * o + 1];
       const int pr1 = m.geom_priority[g1], pr2 = m.geom_priority[g2];
+      const double* fr = env_table(em, e, EF_geom_friction, m.geom_friction);
       int condim; double mu;
-      if (pr1 != pr2) { const int gp = pr1 > pr2 ? g1 : g2; condim = m.geom_condim[gp]; mu = m.geom_friction[3 * gp]; }
-      else { condim = max(m.geom_condim[g1], m.geom_condim[g2]); mu = fmax(m.geom_friction[3 * g1], m.geom_friction[3 * g2]); }
+      if (pr1 != pr2) { const int gp = pr1 > pr2 ? g1 : g2; condim = m.geom_condim[gp]; mu = fr[3 * gp]; }
+      else { condim = max(m.geom_condim[g1], m.geom_condim[g2]); mu = fmax(fr[3 * g1], fr[3 * g2]); }
       const double* ef = io.efc_force + (size_t)e * m.njmax + adr;
       if (condim == 1) f[0] = ef[0];
       else {   // pyramid edges (+t1, -t1, +t2, -t2): mju_decodePyramid
@@ -3395,12 +3480,13 @@ extern "C" __global__ void b200mj_contact_force_kernel(const __grid_constant__ D
 static int launch(const b200mj_model* M, const b200mj_io* io, int batch, int nstep, int flags, int mode, int extra, void* stream,
                   const uint8_t* env_mask = nullptr) {
   if (!M || !io || batch <= 0 || nstep < 0) return -1;
+  if (!env_rows_cover(M, batch)) return -10;
   const_cast<b200mj_model*>(M)->reuse_ok = 0;      // the fused kernel leaves no handover behind
   if (!io->qpos || !io->qvel || (M->dm.na > 0 && !io->act)) return -1;
   int epb = M->envs_per_block;
   int grid = (batch + epb - 1) / epb;
   const size_t smem = M->smem_per_env * epb;
-  B200MJ_LAUNCH(step_kernel_for(M), grid, 32 * epb, smem, (cudaStream_t)stream, M->dm, M->lay, *io, batch, nstep, flags, mode, extra, env_mask);
+  B200MJ_LAUNCH(step_kernel_for(M), grid, 32 * epb, smem, (cudaStream_t)stream, M->dm, M->lay, *io, batch, nstep, flags, mode, extra, env_mask, M->em);
   g_launches++;
   return cudaGetLastError() == cudaSuccess ? 0 : -5;
 }
@@ -3408,6 +3494,7 @@ static int launch(const b200mj_model* M, const b200mj_io* io, int batch, int nst
 int b200mj_step(const b200mj_model* Mc, const b200mj_io* io, int batch, int nstep, int flags, void* stream) {
   b200mj_model* M = const_cast<b200mj_model*>(Mc);
   if (!M || !io || batch <= 0 || nstep < 0) return -1;
+  if (!env_rows_cover(M, batch)) return -10;
   // Split path: Euler, legacy ordering, no applied forces routed in, workspaces fit. Everything else (RK4, the
   // non-legacy ordering, qfrc/xfrc_applied) runs through the fused kernel.
   bool can_split = M->hooks.split && nstep >= 1 && (flags & B200MJ_STEP_LEGACY) && M->dm.integrator == BMJ_INT_EULER &&
@@ -3474,7 +3561,7 @@ int b200mj_step(const b200mj_model* Mc, const b200mj_io* io, int batch, int nste
       if (!(reuse && s == 0)) {
         const Compact cp = compact();
         B200MJ_LAUNCH(pos_kernel_for(M, false), gp, 32 * M->epb_pos, M->smem_pos * M->epb_pos + 64, sm, M->dm, M->lay_pos, M->ho, *io,
-                      e1, flags, last && want_sens, e0, cp);
+                      e1, flags, last && want_sens, e0, cp, M->em);
         g_launches++;
       }
       if (M->nbucket > 1) cudaEventRecord(M->ev_pos[g], sm);
@@ -3491,7 +3578,7 @@ int b200mj_step(const b200mj_model* Mc, const b200mj_io* io, int batch, int nste
         const int grid = (cnt + wpc - 1) / wpc;
         const int* bl = glist + (size_t)b * M->hand_batch;
         const Lay& la = last ? M->lay_accs_b[b] : M->lay_acc_b[b];
-        B200MJ_LAUNCH(acc_kernel_for(M->tn_nv, last), grid, 32 * wpc, ws * wpc, sb, M->dm, la, M->ho, *io, s == 0, flags, gcount + b, bl);
+        B200MJ_LAUNCH(acc_kernel_for(M->tn_nv, last, envm(M)), grid, 32 * wpc, ws * wpc, sb, M->dm, la, M->ho, *io, s == 0, flags, gcount + b, bl, M->em);
         if (b > 0) cudaEventRecord(M->ev_acc[g][b], sb);
         g_launches++;
       }
@@ -3499,7 +3586,7 @@ int b200mj_step(const b200mj_model* Mc, const b200mj_io* io, int batch, int nste
     }
     const Compact cp = compact();      // the lists of the next call's first physics step
     B200MJ_LAUNCH(pos_kernel_for(M, true), gp, 32 * M->epb_pos, M->smem_pos * M->epb_pos + 64, sm, M->dm, M->lay_pos, M->ho, *io,
-                  e1, flags, want_sens && nstep == 1, e0, cp);
+                  e1, flags, want_sens && nstep == 1, e0, cp, M->em);
     g_launches++;
     if (g > 0) { cudaEventRecord(M->ev_join[g], sm); cudaStreamWaitEvent(st, M->ev_join[g], 0); }
   }
@@ -3519,6 +3606,7 @@ int b200mj_forward_masked(const b200mj_model* M, const b200mj_io* io, int batch,
 
 int b200mj_reset(const b200mj_model* M, const b200mj_io* io, int batch, const uint8_t* env_mask, int keyframe, void* stream) {
   if (!M || !io || batch <= 0 || !io->qpos || !io->qvel || (M->dm.na > 0 && !io->act)) return -1;
+  if (!env_rows_cover(M, batch)) return -10;
   const DevModel& m = M->dm;
   const double* key = nullptr;
   if (keyframe >= 0) {
@@ -3535,7 +3623,8 @@ int b200mj_reset(const b200mj_model* M, const b200mj_io* io, int batch, const ui
 
 int b200mj_contact_force(const b200mj_model* M, const b200mj_io* io, int batch, int contact_id, double* out6, void* stream) {
   if (!M || !io || !out6 || batch <= 0) return -1;
-  B200MJ_LAUNCH(b200mj_contact_force_kernel, (batch + 127) / 128, 128, 0, (cudaStream_t)stream, M->dm, *io, batch, contact_id, out6);
+  if (!env_rows_cover(M, batch)) return -10;
+  B200MJ_LAUNCH(b200mj_contact_force_kernel, (batch + 127) / 128, 128, 0, (cudaStream_t)stream, M->dm, *io, batch, contact_id, out6, M->em);
   g_launches++;
   return cudaGetLastError() == cudaSuccess ? 0 : -5;
 }
@@ -3560,9 +3649,30 @@ int b200mj_model_set_variable_geoms(b200mj_model* M, const int32_t* geom_ids, in
   return 0;
 }
 
+int b200mj_model_set_env_fields(b200mj_model* M, const int32_t* field_ids, int n, const double* rows_dev, int nrows) {
+  if (!M || n < 0 || (n > 0 && !field_ids)) return -1;
+  int off[ENV_NFIELDS], row = 0;
+  for (int f = 0; f < ENV_NFIELDS; f++) off[f] = -1;
+  for (int k = 0; k < n; k++) {
+    const int f = (field_ids[k] >= 0 && field_ids[k] < NFIELDS) ? env_field_of(field_ids[k]) : -1;
+    if (f < 0) return -6;
+    if (off[f] >= 0) return -7;
+    off[f] = row; row += M->env_len[f];
+  }
+  if (n > 0 && !rows_dev) return -8;
+  if (n > 0 && nrows < 1) return -9;
+  for (int f = 0; f < ENV_NFIELDS; f++) M->em.off[f] = off[f];
+  M->em.rows = n > 0 ? rows_dev : nullptr; M->em.row = row;
+  M->env_nrows = n > 0 ? nrows : 0;
+  M->reuse_ok = 0;      // the handover left behind was computed with the previous values
+  allow_shared_memory(M);      // (the kernel builds with or without per-environment fields)
+  return 0;
+}
+
 int b200mj_step_host(const b200mj_model* M, const b200mj_io* io, int batch, int nstep, int flags, const double* ctrl_host,
                      double* ctrl_dev, const double* obs_dev, double* obs_host, int nobs, void* stream) {
   if (!M || !io || !ctrl_host || !ctrl_dev) return -1;
+  if (!env_rows_cover(M, batch)) return -10;
   cudaStream_t s = (cudaStream_t)stream;
   if (cudaMemcpyAsync(ctrl_dev, ctrl_host, (size_t)batch * M->dm.nu * sizeof(double), cudaMemcpyHostToDevice, s) != cudaSuccess) return -2;
   b200mj_io io2 = *io; io2.ctrl = ctrl_dev;

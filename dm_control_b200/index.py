@@ -4,7 +4,8 @@ Batched twin of `dm_control/mujoco/index.py` (row names from the model's name ta
 nsensordata` axes via `jnt_qposadr/jnt_dofadr/actuator_actadr/sensor_adr` — index.py:94-100 — and the column names
 `x y z`, `qw qx qy qz`, `xx … zz` — index.py:103-175). Every field keeps its leading batch axis: an indexing
 expression that yields shape `S` in the reference yields `[B, *S]` here. Model-side fields (`named.model.*`) are
-unbatched numpy arrays and index exactly as in the reference.
+unbatched numpy arrays and index exactly as in the reference, except the per-environment model fields
+(`physics.set_env_model_fields`), which index the batched `physics.env_model.<field>` tensor with its leading batch axis.
 """
 from __future__ import annotations
 
@@ -29,13 +30,14 @@ _ROW_KIND = {
     **{f: 'body' for f in ('body_pos', 'body_quat', 'body_ipos', 'body_iquat', 'body_mass', 'body_inertia', 'body_parentid',
                            'body_rootid', 'body_subtreemass')},
     **{f: 'geom' for f in ('geom_size', 'geom_pos', 'geom_quat', 'geom_type', 'geom_bodyid', 'geom_friction', 'geom_rbound',
-                           'geom_condim', 'geom_rgba', 'geom_group')},
+                           'geom_condim', 'geom_rgba', 'geom_group', 'geom_solref', 'geom_solimp')},
     **{f: 'site' for f in ('site_pos', 'site_quat', 'site_size', 'site_bodyid', 'site_rgba', 'site_group')},
     **{f: 'camera' for f in ('cam_pos', 'cam_quat', 'cam_fovy', 'cam_bodyid', 'cam_mode', 'cam_targetbodyid')},
     'mat_rgba': 'material',
     **{f: 'joint' for f in ('jnt_type', 'jnt_range', 'jnt_limited', 'jnt_pos', 'jnt_axis', 'jnt_stiffness', 'jnt_qposadr',
                             'jnt_dofadr', 'jnt_bodyid')},
-    **{f: 'actuator' for f in ('actuator_ctrlrange', 'actuator_gear', 'actuator_ctrllimited')},
+    **{f: 'actuator' for f in ('actuator_ctrlrange', 'actuator_gear', 'actuator_ctrllimited', 'actuator_gainprm',
+                               'actuator_biasprm')},
     'qpos0': 'nq', 'dof_damping': 'nv', 'dof_armature': 'nv',
     **{n: f.rows for n, f in DATA_FIELDS.items() if f.rows},
 }
@@ -104,6 +106,8 @@ class FieldIndexer:
     k = self._translate(key)
     if isinstance(self._a, torch.Tensor):
       self._a[k] = torch.as_tensor(value, dtype=self._a.dtype, device=self._a.device)
+      if self._on_write is not None:
+        self._on_write()          # per-environment model field: the next step recomputes the position stage
     else:
       self._a[k] = value
       if self._on_write is not None:
@@ -118,7 +122,8 @@ class FieldIndexer:
 
 
 class _Struct:
-  def __init__(self, getter, model, batched):
+  def __init__(self, getter, model, batched, dirty=None):
+    object.__setattr__(self, '_dirty', dirty)
     object.__setattr__(self, '_g', getter)
     object.__setattr__(self, '_m', model)
     object.__setattr__(self, '_b', batched)
@@ -130,7 +135,8 @@ class _Struct:
       raise AttributeError(name)
     c = self._cache.get(name)
     if c is None or c._a is not arr:
-      c = FieldIndexer(name, arr, self._m, self._b, on_write=None if self._b else self._m.touch)
+      env = not self._b and isinstance(arr, torch.Tensor)      # a per-environment model field
+      c = FieldIndexer(name, arr, self._m, self._b or env, on_write=self._dirty if env else None if self._b else self._m.touch)
       self._cache[name] = c
     return c
 
@@ -142,6 +148,8 @@ class NamedIndexStructs:
     m = physics.model
 
     def model_get(name):
+      if name in getattr(physics, 'env_model_fields', ()):
+        return getattr(physics.env_model, name)
       a = m.fields.get(name)
       if a is None:
         a = getattr(m, 'vis', {}).get(name)      # colours, groups, cameras: visual tables outside the physics blob
@@ -152,4 +160,4 @@ class NamedIndexStructs:
            'jnt_range': 2, 'actuator_ctrlrange': 2}.get(name)
       return a.reshape(-1, w) if (w and a.ndim == 1) else a
     self.data = _Struct(lambda name: getattr(physics.data, name, None), m, True)
-    self.model = _Struct(model_get, m, False)
+    self.model = _Struct(model_get, m, False, dirty=getattr(physics, 'mark_as_dirty', None))

@@ -40,7 +40,8 @@ STEP_LEGACY, STEP_FULL_FINAL, STEP_SENSORS, STEP_REUSE_POS = 1, 2, 4, 8
 SYMBOLS = ('b200mj_model_create', 'b200mj_model_destroy', 'b200mj_model_set_disableflags', 'b200mj_model_set_capacity',
            'b200mj_step', 'b200mj_forward', 'b200mj_step_host', 'b200mj_workspace_bytes', 'b200mj_envs_per_block', 'b200mj_describe',
            'b200mj_launch_count', 'b200mj_error_string', 'b200mj_version', 'b200mj_reset', 'b200mj_forward_masked',
-           'b200mj_contact_force', 'b200mj_subtree_vel', 'b200mj_model_set_variable_geoms', 'b200mj_render')
+           'b200mj_contact_force', 'b200mj_subtree_vel', 'b200mj_model_set_variable_geoms', 'b200mj_render',
+           'b200mj_model_set_env_fields')
 
 _lib = None
 
@@ -74,9 +75,10 @@ def load():
   L.b200mj_contact_force.argtypes = [vp, ctypes.POINTER(IO), ctypes.c_int, ctypes.c_int, vp, vp]
   L.b200mj_subtree_vel.argtypes = [vp, ctypes.POINTER(IO), ctypes.c_int, ctypes.c_int, vp]
   L.b200mj_model_set_variable_geoms.argtypes = [vp, _c_int_p, ctypes.c_int]
+  L.b200mj_model_set_env_fields.argtypes = [vp, _c_int_p, ctypes.c_int, vp, ctypes.c_int]
   for f in ('b200mj_step', 'b200mj_forward', 'b200mj_step_host', 'b200mj_model_set_disableflags',
             'b200mj_model_set_capacity', 'b200mj_envs_per_block', 'b200mj_reset', 'b200mj_forward_masked', 'b200mj_contact_force',
-            'b200mj_subtree_vel', 'b200mj_model_set_variable_geoms'):
+            'b200mj_subtree_vel', 'b200mj_model_set_variable_geoms', 'b200mj_model_set_env_fields'):
     getattr(L, f).restype = ctypes.c_int
   if hasattr(L, 'b200mj_render'):      # (absent from the CPU emulation build of the physics kernels, tests/emu: no renderer there)
     L.b200mj_render.argtypes = [vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp]

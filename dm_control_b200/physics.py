@@ -102,6 +102,24 @@ DATA_FIELDS = {f.name: f for f in (DataField(*row) for row in (
 STATE_FIELDS = tuple(n for n, f in DATA_FIELDS.items() if f.role == STATE)
 APPLIED_FIELDS = tuple(n for n, f in DATA_FIELDS.items() if f.role == APPLIED)
 
+# model fields an environment may hold values of its own (b200mj_model_set_env_fields, include/b200mj.h): the tables a
+# domain-randomising task varies per episode and from which the engine derives nothing at model creation
+ENV_MODEL_FIELDS = ('body_mass', 'body_inertia', 'body_ipos', 'geom_friction', 'geom_solref', 'geom_solimp', 'dof_damping',
+                    'dof_armature', 'jnt_stiffness', 'actuator_gainprm', 'actuator_biasprm')
+_FIELD_ID = {name: k for k, (name, _) in enumerate(_model.FIELDS)}
+
+
+def check_env_model_fields(names):
+  """Raises ValueError naming the first field of `names` that cannot vary per environment, or that is listed twice."""
+  seen = set()
+  for n in names:
+    if n not in ENV_MODEL_FIELDS:
+      raise ValueError(f'model field {n!r} cannot vary per environment; the per-environment fields are '
+                       f'{", ".join(ENV_MODEL_FIELDS)}')
+    if n in seen:
+      raise ValueError(f'model field {n!r} is listed twice')
+    seen.add(n)
+
 
 class _Data:
   """Batched mjData slice: `[B, ...]` torch tensors, MuJoCo field names."""
@@ -147,6 +165,10 @@ class BatchedPhysics:
     # reference's contract) or mark_as_dirty().
     self._pos_current = False
     self._handle = ctypes.c_void_p()
+    # bumped whenever what a launch captures by value changes (model handle, disable flags, io pointers, per-environment
+    # geoms / model fields): a CUDA graph of a step recorded before that must not be replayed (control.py)
+    self._launch_epoch = 0
+    self._env_model_names, self._env_rows, self.env_model = (), None, None
     self._upload_model()
     self.data = _Data()
     self._io = _lib.IO()
@@ -180,6 +202,7 @@ class BatchedPhysics:
 
   def _upload_model(self):
     self._pos_current = False
+    self._launch_epoch += 1
     if self._handle:
       self._L.b200mj_model_destroy(self._handle)
       self._handle = ctypes.c_void_p()
@@ -192,11 +215,13 @@ class BatchedPhysics:
     self._model_version = self.model._version
     self._model_flags_version = self.model._flags_version
     self._apply_variable_geoms()       # a re-uploaded model forgets its per-environment geom list
+    self._apply_env_model()            # and its per-environment model fields
 
   def _alloc(self, f):
     setattr(self.data, f.name, torch.zeros((self.batch,) + f.shape(self.model), dtype=f.dtype, device=self.device))
 
   def _bind_io(self):
+    self._launch_epoch += 1
     for name, ctype in _lib.IO_FIELDS:
       t = getattr(self.data, name, None)
       if t is None or t.numel() == 0 or (name in APPLIED_FIELDS and not self._applied_on):
@@ -252,9 +277,12 @@ class BatchedPhysics:
     var = getattr(self, '_var_geom_ids', None)
     if var is not None:
       state['var_geom_pos'] = self.data.var_geom_pos.cpu(); state['var_geom_size'] = self.data.var_geom_size.cpu()
-    return dict(model=self.model, batch=self.batch, device=str(self.device), sensors=self._sensors, full_final=self._full_final,
-                legacy_step=self.legacy_step, check_errors=self.check_errors, applied=self._applied_on, var_geom_ids=var, state=state,
-                outputs=[n for n in DATA_FIELDS if hasattr(self.data, n)])
+    st = dict(model=self.model, batch=self.batch, device=str(self.device), sensors=self._sensors, full_final=self._full_final,
+              legacy_step=self.legacy_step, check_errors=self.check_errors, applied=self._applied_on, var_geom_ids=var, state=state,
+              outputs=[n for n in DATA_FIELDS if hasattr(self.data, n)])
+    if self._env_model_names:
+      st['env_model'] = (self._env_model_names, self._env_rows.cpu())
+    return st
 
   def __setstate__(self, st):
     self.__init__(st['model'], batch=st['batch'], device=st['device'], outputs=st['outputs'], sensors=st['sensors'],
@@ -264,6 +292,10 @@ class BatchedPhysics:
       self.enable_applied_forces(True)
     if st['var_geom_ids'] is not None:
       self.set_variable_geoms(st['var_geom_ids'])
+    if 'env_model' in st:
+      names, rows = st['env_model']
+      self.set_env_model_fields(names)
+      self._env_rows.copy_(rows.to(self.device))
     for n, t in st['state'].items():
       getattr(self.data, n).copy_(t.to(self.device))
     self.forward()
@@ -273,6 +305,7 @@ class BatchedPhysics:
       self._upload_model()
     elif self.model._flags_version != self._model_flags_version:
       _lib.check(self._L.b200mj_model_set_disableflags(self._handle, int(self.model.opt.disableflags)))
+      self._launch_epoch += 1
       self._model_flags_version = self.model._flags_version
 
   def copy(self, share_model=False):
@@ -283,6 +316,9 @@ class BatchedPhysics:
     other.check_errors = self.check_errors
     if self._applied_on:
       other.enable_applied_forces(True)
+    if self._env_model_names:
+      other.set_env_model_fields(self._env_model_names)
+      other._env_rows.copy_(self._env_rows)
     for name in self._state_fields():
       getattr(other.data, name).copy_(getattr(self.data, name))
     other.forward()
@@ -438,9 +474,60 @@ class BatchedPhysics:
     self._pos_current = False
 
   def _apply_variable_geoms(self):
+    self._launch_epoch += 1
     ids = getattr(self, '_var_geom_ids', None)
     if ids is not None:
       _lib.check(self._L.b200mj_model_set_variable_geoms(self._handle, ids.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), int(ids.size)))
+
+  def set_env_model_fields(self, names):
+    """Per-environment model fields: each environment reads the listed model fields (of ENV_MODEL_FIELDS) from its
+    own row of one `[B, row]` float64 device buffer instead of the shared model. `physics.env_model.<field>` is the
+    `[B, *model.<field>.shape]` view of that buffer; `bind(kind, names).<attr>` and `named.model.<field>` read and write
+    it for these fields. Fields already per-environment keep their rows; the others start from the model's current
+    values. `set_env_model_fields(())` turns the feature off.
+
+    The reference sets these per `Physics`, e.g. `PhysicsVariator.apply_variations` (composer/variation/__init__.py:90-136);
+    here each environment is one `Physics`. An environment then steps exactly as a BatchedPhysics on a copy of the model
+    with its values written through `model.set`: nothing derived is recomputed (body_subtreemass, the invweight0 tables,
+    stat.meaninertia, the actuator moments keep the shared model's values), and an environment whose `dof_damping` row
+    has a positive entry takes mj_Euler's implicit damping update. While a field is per-environment, its rows are what
+    the engine uses: a write to the shared model's field still re-uploads the model but does not reach the rows. A
+    direct in-place write to `env_model.*` is like one to `data.qpos`: call `forward()` or `mark_as_dirty()` before
+    the next step (writes through `bind` and `named.model` do this)."""
+    names = tuple(names)
+    check_env_model_fields(names)
+    m, B = self.model, self.batch
+    parts = []
+    for n in names:
+      if n in self._env_model_names:
+        parts.append(getattr(self.env_model, n).reshape(B, -1))
+      else:
+        parts.append(torch.as_tensor(np.asarray(m.fields[n], dtype=np.float64).reshape(1, -1), device=self.device).expand(B, -1))
+    if names:
+      self._env_rows = torch.cat(parts, dim=1).contiguous()
+      self.env_model, o = types.SimpleNamespace(), 0
+      for n in names:
+        k = m.fields[n].size
+        setattr(self.env_model, n, self._env_rows[:, o:o + k].view((B,) + m.fields[n].shape))
+        o += k
+    else:
+      self._env_rows, self.env_model = None, None
+    self._env_model_names = names
+    self._apply_env_model()
+    self._pos_current = False
+
+  @property
+  def env_model_fields(self):
+    """The model fields that are per-environment (set_env_model_fields), in row order."""
+    return self._env_model_names
+
+  def _apply_env_model(self):
+    self._launch_epoch += 1
+    names = self._env_model_names
+    ids = np.array([_FIELD_ID[n] for n in names], dtype=np.int32)
+    rows = ctypes.c_void_p(self._env_rows.data_ptr() if names else None)
+    _lib.check(self._L.b200mj_model_set_env_fields(self._handle, ids.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), len(names),
+                                                    rows, self.batch if names else 0))
 
   @contextlib.contextmanager
   def reset_context(self):

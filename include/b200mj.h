@@ -15,6 +15,7 @@
  *   b200mj_contact_force  <- mujoco.mj_contactForce                                           mujoco/wrapper/core.py:546-551
  *   b200mj_subtree_vel    <- mujoco.mj_subtreeVel (after a position/velocity stage)           locomotion/walkers/legacy_base.py:179-186
  *   b200mj_model_set_variable_geoms <- the per-episode recompile of the composer arenas       composer/environment.py:378-383
+ *   b200mj_model_set_env_fields <- per-Physics model writes, e.g. PhysicsVariator.apply_variations   composer/variation/__init__.py:90-136
  *   b200mj_render         <- Physics.render / Camera.render (rgb, depth, segmentation)         mujoco/engine.py:178-233,840-946
  *                            (a ray caster over the model's primitives: hand-off images, not MuJoCo's OpenGL pixels)
  *   b200mj_workspace_bytes / b200mj_envs_per_block / b200mj_describe / b200mj_launch_count : instrumentation
@@ -165,6 +166,15 @@ int b200mj_contact_force(const b200mj_model* m, const b200mj_io* io, int batch, 
 int b200mj_subtree_vel(const b200mj_model* m, const b200mj_io* io, int batch, int flags, void* stream);
 /* Name the geoms that take per-environment pos / size from io->var_geom_pos / var_geom_size (slot k <-> geom_ids[k]). */
 int b200mj_model_set_variable_geoms(b200mj_model* m, const int32_t* geom_ids, int n);
+/* Per-environment model fields: for each environment e < nrows, field field_ids[k] (its position in
+ * B200MJ_MODEL_FIELDS) is read from rows_dev[e * row + off_k] instead of the shared model, where row is the sum of
+ * the listed fields' full lengths in the order given and off_k the sum of the lengths before k. n == 0: off.
+ * Supported (float64): body_mass, body_inertia, body_ipos, geom_friction, geom_solref, geom_solimp, dof_damping,
+ * dof_armature, jnt_stiffness, actuator_gainprm, actuator_biasprm; nothing derived from them is recomputed (MuJoCo's
+ * model-write rule without mj_setConst). An environment whose dof_damping row has a positive entry takes the implicit
+ * damping update of mj_Euler. rows_dev is read by every later call until the next b200mj_model_set_env_fields (a
+ * captured graph reads the live rows); calls that run physics on more than nrows environments return an error. */
+int b200mj_model_set_env_fields(b200mj_model* m, const int32_t* field_ids, int n, const double* rows_dev, int nrows);
 
 /* instrumentation */
 int64_t b200mj_workspace_bytes(const b200mj_model* m);   /* shared memory per environment (bytes) */
