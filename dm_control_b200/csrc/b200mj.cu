@@ -2063,10 +2063,28 @@ __device__ __forceinline__ double newton_gradient(const Ctx& c) {
   return gnorm;
 }
 
+// Compile-time size from TN_ONE_CALL_NV dofs on: the whole direction, and M search and J search for the line search,
+// behind ONE call from the kernel. These kernels are register-bound (128 per thread at 16 warps per SM); every call site
+// of a __noinline__ routine in the Newton loop costs spill code around the call, and an inlined row product keeps N more
+// registers live there (27 dofs: 60 / 88 bytes of spill stores / loads in the kernel body before, none after). The
+// smaller kernels do not spill, and there the extra call only costs (cheetah, 9 dofs: 2 % slower).
+#define TN_ONE_CALL_NV 18
+template <int NVT>
+__device__ __noinline__ void tn_newton_direction(const DevModel& m, const Lay& L, double* ws, int lane, int nefc, int nact, int refactor) {
+  const Ctx c(m, L, ws, lane, 0, 0);
+  if (refactor) tn_factor<NVT>(W(M), W(H), W(dinv), lane, W(grad), W(search), W(J), W(efcSD), reinterpret_cast<const int*>(W(actlist)), nact, W(colbuf));
+  else tn_forward<NVT>(W(H), W(dinv), W(grad), W(search), lane);
+  tn_back<NVT>(W(H), W(dinv), W(search), W(search), lane, 1);
+  if (lane < NVT) W(Mv)[lane] = tn_symv_row<NVT>(W(M), W(search), lane);
+  FOR_LANES(r, nefc) W(jv)[r] = tn_dot_row<NVT>(W(J) + r * (NVT | 1), W(search));
+  __syncwarp();
+}
+
 template <int NVT>
 __device__ __forceinline__ void newton_direction(const Ctx& c, int nefc, int nact, bool refactor) {
   const DevModel& m = c.m; int lane = c.lane; int nv = m.nv, ld = m.ldv;
   if constexpr (NVT == 0) { if (c.L.dual) { newton_direction_dual(c, nefc, nact, refactor); return; } }
+  if constexpr (NVT >= TN_ONE_CALL_NV) { tn_newton_direction<NVT>(c.m, c.L, c.ws, lane, nefc, nact, refactor); return; }
   if constexpr (NVT > 0) {
     if (refactor) tn_factor<NVT>(W(M), W(H), W(dinv), lane, W(grad), W(search), W(J), W(efcSD), reinterpret_cast<const int*>(W(actlist)), nact, W(colbuf));
     else tn_forward<NVT>(W(H), W(dinv), W(grad), W(search), lane);
@@ -2126,11 +2144,12 @@ __device__ __forceinline__ double line_search(const Ctx& c, int nefc, const Prim
   double g1 = 0, g2 = 0;
   if constexpr (NVT > 0) {
     if (lane < NVT) {
-      double s = tn_symv_row<NVT>(W(M), W(search), lane);
-      W(Mv)[lane] = s;
+      double s;
+      if constexpr (NVT >= TN_ONE_CALL_NV) s = W(Mv)[lane];      // tn_newton_direction
+      else { s = tn_symv_row<NVT>(W(M), W(search), lane); W(Mv)[lane] = s; }
       g1 += W(search)[lane] * (W(Ma)[lane] - W(smooth)[lane]); g2 += 0.5 * W(search)[lane] * s;
     }
-    FOR_LANES(r, nefc) W(jv)[r] = tn_dot_row<NVT>(W(J) + r * ld, W(search));
+    if constexpr (NVT < TN_ONE_CALL_NV) { FOR_LANES(r, nefc) W(jv)[r] = tn_dot_row<NVT>(W(J) + r * ld, W(search)); }
   } else {
     const bool have_mv = c.L.dual != 0;      // the dual form of the direction delivers M search as well (newton_direction_dual)
     FOR_LANES(i, nv) {
