@@ -21,28 +21,39 @@ import numpy as np
 import torch
 
 from . import index
+from .model import MODEL_FIELDS
 from .physics import DATA_FIELDS, STATE
 
-_PREFIX = dict(body='body_', geom='geom_', site='site_', joint='jnt_', actuator='actuator_', sensor='sensor_', tendon='tendon_',
-               dof='dof_')
 # model fields a joint reaches through its dofs (mjcf/physics.py binds a joint's `damping` / `armature` to dof_damping /
 # dof_armature the same way): ragged, one column per dof of the bound joints
 _MODEL_ALIAS = {'joint': {'damping': 'dof_damping', 'armature': 'dof_armature'}}
+# (row axis, attribute) -> model field: `geom_pos` is a geom's `pos`, `jnt_range` a joint's `range`
+_MODEL_ATTR = {(f.rows, n.split('_', 1)[1]): n for n, f in MODEL_FIELDS.items() if '_' in n}
 _DATA_ALIAS = {'geom': {'xpos': 'geom_xpos', 'xmat': 'geom_xmat'}, 'site': {'xpos': 'site_xpos', 'xmat': 'site_xmat'},
                'actuator': {'force': 'actuator_force'}}
 
 
 def model_field(kind, attr):
-  """The model field behind attribute `attr` of a bound `kind` element."""
-  return _MODEL_ALIAS.get(kind, {}).get(attr, _PREFIX[kind] + attr)
+  """The model field behind attribute `attr` of a bound `kind` element (`<kind>_<attr>` where there is none)."""
+  return _MODEL_ALIAS.get(kind, {}).get(attr) or _MODEL_ATTR.get((kind, attr), f'{kind}_{attr}')
 
 
-def model_rows(model, kind, field, ids):
-  """(ragged, rows of `field` that belong to the elements `ids` of `kind`): a joint's dofs for the dof fields."""
-  if field.startswith('dof_') and kind == 'joint':
-    slices = index._ragged(model, 'nv')
-    return True, [c for i in ids for c in range(slices[i].start, slices[i].stop)]
-  return False, [int(i) for i in ids]
+def element_rows(model, axis, kind, ids):
+  """(ragged, indices along row axis `axis` that belong to the elements `ids` of `kind`): the columns of their slices
+  of a ragged axis (the slices `physics.named` uses), or their rows; None where `axis` is not `kind`'s."""
+  if axis in index._RAGGED_AXES and index._RAGGED_AXES[axis][0] == kind:
+    slices = index._ragged(model, axis)
+    return True, [c for i in ids if slices[i] is not None for c in range(slices[i].start, slices[i].stop)]
+  return (False, [int(i) for i in ids]) if axis == kind else None
+
+
+def model_rows(model, kind, attr, ids):
+  """(field, ragged, rows) of the model field behind attribute `attr` of the elements `ids` of `kind` (element_rows)."""
+  field = model_field(kind, attr)
+  found = field in MODEL_FIELDS and element_rows(model, MODEL_FIELDS[field].rows, kind, ids)
+  if not found:
+    raise AttributeError(f'bound {kind} has no attribute {attr!r}')
+  return (field,) + found
 
 
 class Binding:
@@ -60,28 +71,17 @@ class Binding:
     object.__setattr__(self, '_tids', torch.as_tensor(ids, device=physics.device))
 
   # ---- helpers ----
-  def _index(self, name, field):
-    """(ragged, indices along axis 1 of `data.<field>`) of the bound elements: the columns of their slices of a ragged
-    field (the slices `physics.named` uses), or their rows of a per-element field."""
-    rows = DATA_FIELDS[field].rows if field in DATA_FIELDS else None
-    if rows in index._RAGGED_AXES and index._RAGGED_AXES[rows][0] == self._kind:
-      slices = index._ragged(self._p.model, rows)
-      cols = [c for i in self._ids if slices[i] is not None for c in range(slices[i].start, slices[i].stop)]
-      return True, torch.tensor(cols, dtype=torch.int64, device=self._p.device)
-    if rows == self._kind:
-      return False, self._tids
-    raise AttributeError(f'{name!r} is not a per-{self._kind} data field')
-
-  def _data_field(self, name):
-    d = self._p.data
-    name = _DATA_ALIAS.get(self._kind, {}).get(name, name)
-    t = getattr(d, name, None)
-    return (name, t) if isinstance(t, torch.Tensor) else (name, None)
-
-  def _env_rows(self, mname):
-    """[B, n, w] view of a per-environment model field (physics.set_env_model_fields)."""
-    t = getattr(self._p.env_model, mname)
-    return t.reshape(t.shape[0], t.shape[1], -1)
+  def _data(self, name):
+    """(field, tensor, ragged, indices along axis 1) of the data field behind `name` for the bound elements
+    (element_rows); None where `name` is no data field of this kind."""
+    field = _DATA_ALIAS.get(self._kind, {}).get(name, name)
+    t = getattr(self._p.data, field, None)
+    found = (isinstance(t, torch.Tensor) and field in DATA_FIELDS and
+             element_rows(self._p.model, DATA_FIELDS[field].rows, self._kind, self._ids))
+    if not found:
+      return None
+    ragged, idx = found
+    return field, t, ragged, torch.tensor(idx, dtype=torch.int64, device=self._p.device) if ragged else self._tids
 
   def _squeeze(self, t):
     return t[:, 0] if self._single and t.dim() >= 2 else t
@@ -89,36 +89,26 @@ class Binding:
   # ---- attribute access ----
   def __getattr__(self, name):
     p = self._p
-    field, t = self._data_field(name)
-    if t is not None:
-      ragged, idx = self._index(name, field)
+    data = self._data(name)
+    if data is not None:
+      field, t, ragged, idx = data
       if DATA_FIELDS[field].role != STATE and getattr(p, '_bind_dirty', False):
         p.forward()                              # lazily, once: derived quantities after a state write through a binding
       out = t.index_select(1, idx)
       return out if ragged else self._squeeze(out)
-    mname = model_field(self._kind, name)
-    if mname in getattr(p, 'env_model_fields', ()):          # per-environment model field: [B, k(, w)]
-      ragged, rows = model_rows(p.model, self._kind, mname, self._ids)
-      out = self._env_rows(mname)[:, torch.as_tensor(rows, dtype=torch.int64, device=p.device)]
-      out = out[..., 0] if out.shape[2] == 1 else out
+    field, ragged, idx = model_rows(p.model, self._kind, name, self._ids)
+    if field in getattr(p, 'env_model_fields', ()):          # per-environment model field: [B, k(, w)]
+      out = getattr(p.env_model, field)[:, torch.as_tensor(idx, dtype=torch.int64, device=p.device)]
       return out if ragged else self._squeeze(out)
-    arr = p.model.fields.get(mname)
-    if arr is None:
-      raise AttributeError(f'bound {self._kind} has no attribute {name!r}')
-    ragged, idx = model_rows(p.model, self._kind, mname, self._ids)
-    if ragged:
-      return np.asarray(arr)[idx]
-    n = len(p.model.ordered_names[self._kind]) if self._kind in p.model.ordered_names else arr.shape[0]
-    rows = np.asarray(arr).reshape(n, -1)[idx]
-    rows = rows[:, 0] if rows.shape[1] == 1 else rows
-    return rows[0] if self._single else rows
+    out = p.model.fields[field][idx]
+    return out[0] if self._single and not ragged else out
 
   def __setattr__(self, name, value):
     p = self._p
-    field, t = self._data_field(name)
-    if t is not None:
+    data = self._data(name)
+    if data is not None:
+      field, t, ragged, idx = data
       v = torch.as_tensor(value, dtype=t.dtype, device=p.device)
-      ragged, idx = self._index(name, field)
       if ragged:
         t[:, idx] = v
       else:
@@ -130,10 +120,10 @@ class Binding:
         if field != 'ctrl':                      # ctrl does not invalidate position / velocity-stage quantities
           object.__setattr__(p, '_bind_dirty', True)
       return
-    mname = model_field(self._kind, name)
-    if mname in getattr(p, 'env_model_fields', ()):          # per-environment model field: [B, k, w], [k, w] or a scalar
-      rows = self._env_rows(mname)
-      _, idx = model_rows(p.model, self._kind, mname, self._ids)
+    field, ragged, idx = model_rows(p.model, self._kind, name, self._ids)
+    if field in getattr(p, 'env_model_fields', ()):          # per-environment model field: [B, k, w], [k, w] or a scalar
+      rows = getattr(p.env_model, field)
+      rows = rows.reshape(rows.shape[0], rows.shape[1], -1)    # [B, n, w]
       tidx = torch.as_tensor(idx, dtype=torch.int64, device=p.device)
       k, w = len(idx), rows.shape[2]
       v = torch.as_tensor(value, dtype=rows.dtype, device=p.device)
@@ -145,16 +135,10 @@ class Binding:
       p.mark_as_dirty()
       object.__setattr__(p, '_bind_dirty', True)
       return
-    if mname not in p.model.fields:
-      raise AttributeError(f'bound {self._kind} has no attribute {name!r}')
-    arr = p.model.fields[mname]
-    ragged, idx = model_rows(p.model, self._kind, mname, self._ids)
+    arr = p.model.fields[field]
     if ragged:
       arr[idx] = np.asarray(value, dtype=arr.dtype)
-      p.model.touch()
-      object.__setattr__(p, '_bind_dirty', True)
-      return
-    n = len(p.model.ordered_names[self._kind])
-    arr.reshape(n, -1)[self._ids] = np.asarray(value, dtype=arr.dtype).reshape(len(self._ids), -1) if np.ndim(value) else value
+    else:                                        # [n, w]: k rows, or one row for all
+      arr.reshape(arr.shape[0], -1)[idx] = np.asarray(value, dtype=arr.dtype).reshape(len(idx), -1) if np.ndim(value) else value
     p.model.touch()
     object.__setattr__(p, '_bind_dirty', True)

@@ -12,34 +12,21 @@ from __future__ import annotations
 import numpy as np
 import torch
 
+from .model import MODEL_FIELDS
 from .physics import DATA_FIELDS
 
 _COLS = {'xyz': ['x', 'y', 'z'], 'quat': ['qw', 'qx', 'qy', 'qz'], 'mat': ['xx', 'xy', 'xz', 'yx', 'yy', 'yz', 'zx', 'zy', 'zz'],
          'rgba': ['r', 'g', 'b', 'a']}
-# field -> kind of its column names; the data fields' come from physics.DATA_FIELDS
-_COL_KIND = {
-    **dict.fromkeys(('body_pos', 'body_ipos', 'body_inertia', 'jnt_pos', 'jnt_axis', 'geom_size', 'geom_pos', 'site_size',
-                     'site_pos'), 'xyz'),
-    **dict.fromkeys(('body_quat', 'body_iquat', 'geom_quat', 'site_quat'), 'quat'),
-    **dict.fromkeys(('geom_rgba', 'site_rgba', 'mat_rgba'), 'rgba'),      # index.py:103-175 `rgba`; visual tables, Model.vis
-    **{n: f.cols for n, f in DATA_FIELDS.items() if f.cols},
-}
-
-# field -> kind of its row axis; the data fields' come from physics.DATA_FIELDS
+_FIELDS = {**MODEL_FIELDS, **DATA_FIELDS}
+# field -> kind of its column names; the visual tables (Model.vis) are not blob fields
+_COL_KIND = {**dict.fromkeys(('geom_rgba', 'site_rgba', 'mat_rgba'), 'rgba'),      # index.py:103-175 `rgba`
+             **{n: f.cols for n, f in _FIELDS.items() if f.cols}}
+# field -> kind of its row axis
 _ROW_KIND = {
-    **{f: 'body' for f in ('body_pos', 'body_quat', 'body_ipos', 'body_iquat', 'body_mass', 'body_inertia', 'body_parentid',
-                           'body_rootid', 'body_subtreemass')},
-    **{f: 'geom' for f in ('geom_size', 'geom_pos', 'geom_quat', 'geom_type', 'geom_bodyid', 'geom_friction', 'geom_rbound',
-                           'geom_condim', 'geom_rgba', 'geom_group', 'geom_solref', 'geom_solimp')},
-    **{f: 'site' for f in ('site_pos', 'site_quat', 'site_size', 'site_bodyid', 'site_rgba', 'site_group')},
+    **{f: 'geom' for f in ('geom_rgba', 'geom_group')}, **{f: 'site' for f in ('site_rgba', 'site_group')},
     **{f: 'camera' for f in ('cam_pos', 'cam_quat', 'cam_fovy', 'cam_bodyid', 'cam_mode', 'cam_targetbodyid')},
     'mat_rgba': 'material',
-    **{f: 'joint' for f in ('jnt_type', 'jnt_range', 'jnt_limited', 'jnt_pos', 'jnt_axis', 'jnt_stiffness', 'jnt_qposadr',
-                            'jnt_dofadr', 'jnt_bodyid')},
-    **{f: 'actuator' for f in ('actuator_ctrlrange', 'actuator_gear', 'actuator_ctrllimited', 'actuator_gainprm',
-                               'actuator_biasprm')},
-    'qpos0': 'nq', 'dof_damping': 'nv', 'dof_armature': 'nv',
-    **{n: f.rows for n, f in DATA_FIELDS.items() if f.rows},
+    **{n: f.rows for n, f in _FIELDS.items() if f.rows},
 }
 
 # ragged axis -> (element kind that owns its slices, address table)
@@ -66,7 +53,7 @@ class FieldIndexer:
       names = model.ordered_names[_RAGGED_AXES[kind][0]]
       self._rows = {n: s for n, s in zip(names, _ragged(model, kind)) if s is not None}
     else:
-      self._rows = {n: i for i, n in enumerate(model.ordered_names.get(kind, []))}
+      self._rows = dict(model.names.get(kind, {}))       # name -> id
     self._cols = {c: i for i, c in enumerate(_COLS.get(_COL_KIND.get(name), []))}
 
   def _row_key(self, k):
@@ -151,13 +138,7 @@ class NamedIndexStructs:
       if name in getattr(physics, 'env_model_fields', ()):
         return getattr(physics.env_model, name)
       a = m.fields.get(name)
-      if a is None:
-        a = getattr(m, 'vis', {}).get(name)      # colours, groups, cameras: visual tables outside the physics blob
-      if a is None:
-        return None
-      w = {'body_pos': 3, 'body_quat': 4, 'body_ipos': 3, 'body_iquat': 4, 'body_inertia': 3, 'geom_size': 3, 'geom_pos': 3,
-           'geom_quat': 4, 'geom_friction': 3, 'site_pos': 3, 'site_quat': 4, 'site_size': 3, 'jnt_pos': 3, 'jnt_axis': 3,
-           'jnt_range': 2, 'actuator_ctrlrange': 2}.get(name)
-      return a.reshape(-1, w) if (w and a.ndim == 1) else a
+      # colours, groups, cameras: visual tables outside the physics blob
+      return a if a is not None else getattr(m, 'vis', {}).get(name)
     self.data = _Struct(lambda name: getattr(physics.data, name, None), m, True)
     self.model = _Struct(model_get, m, False, dirty=getattr(physics, 'mark_as_dirty', None))

@@ -48,7 +48,7 @@ class CMUWalker:
     self.nonfoot_geom = torch.as_tensor(np.array([(int(b) in walker_bodies) and (int(b) not in foot_bodies) for b in gb]), device=device)
     self.ground_geom = m.name2id('ground_plane', 'geom')
     # observable joints = the joint of every actuator, in actuator (alphabetical) order (cmu_humanoid.py:337-340)
-    trn = np.asarray(m.actuator_trnid).reshape(-1)[:m.nu] if np.asarray(m.actuator_trnid).ndim == 1 else np.asarray(m.actuator_trnid)[:, 0]
+    trn = np.asarray(m.actuator_trnid)
     self.joint_qpos = torch.as_tensor(np.asarray(m.jnt_qposadr)[trn].astype(np.int64), device=device)
     self.joint_dof = torch.as_tensor(np.asarray(m.jnt_dofadr)[trn].astype(np.int64), device=device)
     names = m.ordered_names['sensor']

@@ -732,17 +732,16 @@ def _finish(c, root, nconmax, njmax):
   F.update(jnt_type=np.array([j['type'] for j in J], np.int32), jnt_qposadr=jnt_qposadr, jnt_dofadr=jnt_dofadr,
            jnt_bodyid=np.array([j['body'] for j in J], np.int32),
            jnt_limited=np.array([j['limited'] for j in J], np.int32),
-           jnt_pos=_arr([j['pos'] for j in J], 3), jnt_axis=_arr([j['axis'] for j in J], 3),
+           jnt_pos=[j['pos'] for j in J], jnt_axis=[j['axis'] for j in J],
            jnt_stiffness=np.array([j['stiffness'] for j in J], np.float64),
-           jnt_range=_arr([j['range'] for j in J], 2), jnt_margin=np.array([j['margin'] for j in J], np.float64),
-           jnt_solref=_arr([j['solref'] for j in J], 2), jnt_solimp=_arr([j['solimp'] for j in J], 5),
+           jnt_range=[j['range'] for j in J], jnt_margin=np.array([j['margin'] for j in J], np.float64),
+           jnt_solref=[j['solref'] for j in J], jnt_solimp=[j['solimp'] for j in J],
            qpos0=np.array(qpos0, np.float64), qpos_spring=np.array(qpos_spring, np.float64))
   F.update(dof_bodyid=dof_body, dof_jntid=dof_jnt, dof_parentid=dof_parent,
            dof_armature=np.array([J[j]['armature'] for j in dof_jnt], np.float64),
            dof_damping=np.array([J[j]['damping'] for j in dof_jnt], np.float64),
            dof_frictionloss=np.array([J[j]['frictionloss'] for j in dof_jnt], np.float64),
-           dof_solref=_arr([J[j]['solreffriction'] for j in dof_jnt], 2),
-           dof_solimp=_arr([J[j]['solimpfriction'] for j in dof_jnt], 5))
+           dof_solref=[J[j]['solreffriction'] for j in dof_jnt], dof_solimp=[J[j]['solimpfriction'] for j in dof_jnt])
 
   G = c.geoms
   F.update(geom_type=np.array([g['type'] for g in G], np.int32), geom_bodyid=np.array([g['body'] for g in G], np.int32),
@@ -750,17 +749,15 @@ def _finish(c, root, nconmax, njmax):
            geom_contype=np.array([g['contype'] for g in G], np.int32),
            geom_conaffinity=np.array([g['conaffinity'] for g in G], np.int32),
            geom_priority=np.array([g['priority'] for g in G], np.int32),
-           geom_size=_arr([g['size'] for g in G], 3), geom_pos=_arr([g['pos'] for g in G], 3),
-           geom_quat=_arr([g['quat'] for g in G], 4),
+           geom_size=[g['size'] for g in G], geom_pos=[g['pos'] for g in G], geom_quat=[g['quat'] for g in G],
            geom_rbound=np.array([_geom_rbound(g['type'], g['size']) for g in G], np.float64),
-           geom_friction=_arr([g['friction'] for g in G], 3), geom_solmix=np.array([g['solmix'] for g in G], np.float64),
-           geom_solref=_arr([g['solref'] for g in G], 2), geom_solimp=_arr([g['solimp'] for g in G], 5),
+           geom_friction=[g['friction'] for g in G], geom_solmix=np.array([g['solmix'] for g in G], np.float64),
+           geom_solref=[g['solref'] for g in G], geom_solimp=[g['solimp'] for g in G],
            geom_margin=np.array([g['margin'] for g in G], np.float64),
            geom_gap=np.array([g['gap'] for g in G], np.float64))
   S = c.sites
   F.update(site_bodyid=np.array([s['body'] for s in S], np.int32), site_type=np.array([s['type'] for s in S], np.int32),
-           site_pos=_arr([s['pos'] for s in S], 3), site_quat=_arr([s['quat'] for s in S], 4),
-           site_size=_arr([s['size'] for s in S], 3))
+           site_pos=[s['pos'] for s in S], site_quat=[s['quat'] for s in S], site_size=[s['size'] for s in S])
 
   # ---- contact candidate pairs (static filters applied once) -------------------------------
   excludes = set()
@@ -853,8 +850,8 @@ def _finish(c, root, nconmax, njmax):
                       solref=_floats(a.get('solref', '0.02 1'), 2), solimp=_solimp(a.get('solimp'))))
   F.update(eq_type=np.array([e['type'] for e in eqs], np.int32), eq_obj1id=np.array([e['o1'] for e in eqs], np.int32),
            eq_obj2id=np.array([e['o2'] for e in eqs], np.int32),
-           eq_active0=np.array([e['active'] for e in eqs], np.int32), eq_data=_arr([e['data'] for e in eqs], 11),
-           eq_solref=_arr([e['solref'] for e in eqs], 2), eq_solimp=_arr([e['solimp'] for e in eqs], 5))
+           eq_active0=np.array([e['active'] for e in eqs], np.int32), eq_data=[e['data'] for e in eqs],
+           eq_solref=[e['solref'] for e in eqs], eq_solimp=[e['solimp'] for e in eqs])
 
   # ---- actuators --------------------------------------------------------------------------
   acts = []
@@ -917,11 +914,10 @@ def _finish(c, root, nconmax, njmax):
            actuator_actlimited=np.array([a['actlimited'] for a in acts], np.int32),
            actuator_actadr=np.array(actadr, np.int32),
            actuator_gear=np.array([a['gear'] for a in acts], np.float64),
-           actuator_gainprm=_arr([a['gainprm'] for a in acts], 3), actuator_biasprm=_arr([a['biasprm'] for a in acts], 3),
+           actuator_gainprm=[a['gainprm'] for a in acts], actuator_biasprm=[a['biasprm'] for a in acts],
            actuator_dynprm=np.array([a['dynprm'] for a in acts], np.float64),
-           actuator_ctrlrange=_arr([a['ctrlrange'] for a in acts], 2),
-           actuator_forcerange=_arr([a['forcerange'] for a in acts], 2),
-           actuator_actrange=_arr([a['actrange'] for a in acts], 2))
+           actuator_ctrlrange=[a['ctrlrange'] for a in acts], actuator_forcerange=[a['forcerange'] for a in acts],
+           actuator_actrange=[a['actrange'] for a in acts])
 
   # ---- sensors ----------------------------------------------------------------------------
   sens = []
@@ -968,7 +964,7 @@ def _finish(c, root, nconmax, njmax):
         kq = _floats(k.attrib['qpos'], nq)
       c.names['key'][k.attrib.get('name', f'_key{len(keys)}')] = len(keys)
       keys.append(kq)
-  F['key_qpos'] = _arr(keys, nq)
+  F['key_qpos'] = keys
 
   # ---- sizes / capacities -----------------------------------------------------------------
   size_node = root.find('size')
@@ -1084,12 +1080,6 @@ def _visual_tables(c, root, F, G, S):
       cam_poscom0=cam_poscom0, cam_mat0=cam_mat0,
       mat_rgba=np.array([c.material_rgba[n] for n in c.materials], dtype=np.float32).reshape(-1, 4),
       global_fovy=np.array([fovy0]), stat_center=np.asarray(center, dtype=np.float64), stat_extent=np.array([extent]))
-
-
-def _arr(rows, width):
-  if len(rows) == 0:
-    return np.zeros((0, width), np.float64)
-  return np.array(rows, dtype=np.float64).reshape(len(rows), width)
 
 
 # ---------------------------------------------------------------------------------------------

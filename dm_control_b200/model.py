@@ -10,6 +10,7 @@ from __future__ import annotations
 import os
 import re
 import types
+from typing import NamedTuple
 
 import numpy as np
 
@@ -39,6 +40,45 @@ OPTR = {n[len('BMJ_OPT_'):]: i for i, n in enumerate(_OPTR[:-1])}
 NOPTR = len(_OPTR) - 1
 OPTI = {n[len('BMJ_OPT_'):]: i for i, n in enumerate(_OPTI[:-1])}
 NOPTI = len(_OPTI) - 1
+
+
+class ModelField(NamedTuple):
+  """One blob field of the compiled model, in the header's order."""
+  name: str
+  dtype: type        # np.int32 or np.float64
+  rows: str | None   # row axis: element kind ('body', ..., 'key'), ragged axis ('nq', 'nv'), unnamed count or None
+  width: tuple = ()  # per-row shape: constants and model sizes by name
+  cols: str | None = None   # column names of index.py: 'xyz' or 'quat'
+  env: int | None = None    # position among the per-environment fields (ENV_FIELDS, csrc/b200mj.cu)
+
+  def shape(self, m):
+    count = () if self.rows is None else (getattr(m, _COUNT[self.rows]) if self.rows in _COUNT else -1,)
+    return count + tuple(getattr(m, d) if isinstance(d, str) else d for d in self.width)
+
+
+# row axis by name prefix where it is not the prefix itself (`body_pos` has one row per body, `pair_geom1` per pair)
+_AXIS = dict(jnt='joint', dof='nv', eq='equality', qpos0='nq', qpos='nq', sizes=None, opt=None)
+# the size that counts a row axis; the levels have none (`level_adr` has nlevel + 1 entries, `level_body` nbody)
+_COUNT = dict(body='nbody', joint='njnt', geom='ngeom', site='nsite', actuator='nu', tendon='ntendon', equality='neq',
+              sensor='nsensor', key='nkey', nq='nq', nv='nv', pair='npair', wrap='nwrap')
+_XYZ, _QUAT, _W2, _W5 = dict(width=(3,), cols='xyz'), dict(width=(4,), cols='quat'), dict(width=(2,)), dict(width=(5,))
+# how each field differs from one value per row
+_DECLARED = {
+    'sizes': dict(width=(NSIZES,)), 'opt_real': dict(width=(NOPTR,)), 'opt_int': dict(width=(NOPTI,)),
+    'body_pos': _XYZ, 'body_quat': _QUAT, 'body_ipos': dict(_XYZ, env=2), 'body_iquat': _QUAT, 'body_mass': dict(env=0),
+    'body_inertia': dict(_XYZ, env=1), 'body_invweight0': _W2, 'body_dofmask': _W2,
+    'jnt_pos': _XYZ, 'jnt_axis': _XYZ, 'jnt_stiffness': dict(env=8), 'jnt_range': _W2, 'jnt_solref': _W2, 'jnt_solimp': _W5,
+    'dof_armature': dict(env=7), 'dof_damping': dict(env=6), 'dof_solref': _W2, 'dof_solimp': _W5,
+    'geom_size': _XYZ, 'geom_pos': _XYZ, 'geom_quat': _QUAT, 'geom_friction': dict(width=(3,), env=3),
+    'geom_solref': dict(_W2, env=4), 'geom_solimp': dict(_W5, env=5),
+    'site_pos': _XYZ, 'site_quat': _QUAT, 'site_size': _XYZ,
+    'actuator_gainprm': dict(width=(3,), env=9), 'actuator_biasprm': dict(width=(3,), env=10), 'actuator_ctrlrange': _W2,
+    'actuator_forcerange': _W2, 'actuator_actrange': _W2,
+    'eq_data': dict(width=(11,)), 'eq_solref': _W2, 'eq_solimp': _W5,
+    'key_qpos': dict(width=('nq',)),
+}
+MODEL_FIELDS = {name: ModelField(name, np.int32 if kind == 'i' else np.float64, _AXIS.get(prefix, prefix), **_DECLARED.get(name, {}))
+                for name, kind in FIELDS for prefix in [name.split('_')[0]]}
 
 # MuJoCo mjtObj names accepted by name2id/id2name (reference: wrapper/core.py:334-387)
 _OBJ_ALIASES = dict(body='body', xbody='body', joint='joint', geom='geom', site='site', actuator='actuator',
@@ -93,9 +133,12 @@ class Model:
     # visual-only tables (colours, groups, cameras, extent): rendering hand-off, never part of the physics blob
     self.vis = {k: np.asarray(v) for k, v in (vis or {}).items()}
     self.fields = {}
-    for name, kind in FIELDS:
-      arr = np.ascontiguousarray(fields[name], dtype=np.int32 if kind == 'i' else np.float64)
-      self.fields[name] = arr
+    for f in MODEL_FIELDS.values():     # `sizes` comes first: the other shapes read it
+      arr = np.ascontiguousarray(fields[f.name], dtype=f.dtype)
+      try:
+        self.fields[f.name] = arr.reshape(f.shape(self))
+      except ValueError:
+        raise ValueError(f'model field {f.name!r}: {arr.size} values do not make its shape {f.shape(self)}') from None
     self.names = names
     self.ordered_names = ordered_names
     self.opt = _Opt(self)

@@ -104,8 +104,8 @@ APPLIED_FIELDS = tuple(n for n, f in DATA_FIELDS.items() if f.role == APPLIED)
 
 # model fields an environment may hold values of its own (b200mj_model_set_env_fields, include/b200mj.h): the tables a
 # domain-randomising task varies per episode and from which the engine derives nothing at model creation
-ENV_MODEL_FIELDS = ('body_mass', 'body_inertia', 'body_ipos', 'geom_friction', 'geom_solref', 'geom_solimp', 'dof_damping',
-                    'dof_armature', 'jnt_stiffness', 'actuator_gainprm', 'actuator_biasprm')
+ENV_MODEL_FIELDS = tuple(f.name for f in sorted((f for f in _model.MODEL_FIELDS.values() if f.env is not None),
+                                                 key=lambda f: f.env))
 _FIELD_ID = {name: k for k, (name, _) in enumerate(_model.FIELDS)}
 
 
@@ -465,8 +465,8 @@ class BatchedPhysics:
     ids = np.ascontiguousarray(geom_ids, dtype=np.int32)
     m, B = self.model, self.batch
     self._var_geom_ids = ids
-    gp = torch.as_tensor(np.array(m.geom_pos, dtype=np.float64).reshape(-1, 3)[ids], device=self.device)
-    gs = torch.as_tensor(np.array(m.geom_size, dtype=np.float64).reshape(-1, 3)[ids], device=self.device)
+    gp = torch.as_tensor(m.geom_pos[ids], device=self.device)
+    gs = torch.as_tensor(m.geom_size[ids], device=self.device)
     self.data.var_geom_pos = gp[None].repeat(B, 1, 1).contiguous()
     self.data.var_geom_size = gs[None].repeat(B, 1, 1).contiguous()
     self._apply_variable_geoms()

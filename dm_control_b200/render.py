@@ -94,7 +94,7 @@ class Camera:
     group = np.concatenate([vis['geom_group'], vis['site_group'][:ns]])
     self._rgba = torch.as_tensor(rgba, device=dev).contiguous()
     self._visible = torch.as_tensor((np.isin(group, list(groups)) & (rgba[:, 3] > 0)).astype(np.uint8), device=dev)
-    self._size_shared = torch.as_tensor(np.concatenate([m.geom_size.reshape(-1, 3), m.site_size.reshape(-1, 3)[:ns]]).astype(np.float64),
+    self._size_shared = torch.as_tensor(np.concatenate([m.geom_size, m.site_size[:ns]]).astype(np.float64),
                                         device=dev).contiguous()
     self._extent = float(vis['stat_extent'][0])
     self._free_pose = Pose(lookat=np.asarray(vis['stat_center'], dtype=np.float64).copy(), distance=1.5 * self._extent,
@@ -216,10 +216,10 @@ def scene_state(physics, env_ids=None):
   m, d, B = physics.model, physics.data, physics.batch
   idx = torch.arange(B, device=physics.device) if env_ids is None else torch.as_tensor(env_ids, device=physics.device)
   take = lambda t, shape: t.index_select(0, idx).reshape((len(idx),) + shape).cpu().numpy()
-  out = dict(geom_type=np.asarray(m.geom_type), geom_size=np.asarray(m.geom_size).reshape(-1, 3), geom_rgba=m.vis['geom_rgba'],
+  out = dict(geom_type=np.asarray(m.geom_type), geom_size=np.asarray(m.geom_size), geom_rgba=m.vis['geom_rgba'],
              geom_xpos=take(d.geom_xpos, (m.ngeom, 3)), geom_xmat=take(d.geom_xmat, (m.ngeom, 9)))
   if m.nsite and hasattr(d, 'site_xpos'):
-    out.update(site_type=np.asarray(m.site_type), site_size=np.asarray(m.site_size).reshape(-1, 3), site_rgba=m.vis['site_rgba'],
+    out.update(site_type=np.asarray(m.site_type), site_size=np.asarray(m.site_size), site_rgba=m.vis['site_rgba'],
                site_xpos=take(d.site_xpos, (m.nsite, 3)), site_xmat=take(d.site_xmat, (m.nsite, 9)))
   ncam = int(m.vis['cam_bodyid'].shape[0])
   if ncam:

@@ -66,22 +66,18 @@ class PhysicsVariator:
       single = isinstance(names, str)
       ids = [m.name2id(x, kind) for x in ([names] if single else names)]
       for attr, info in attrs.items():
-        field = model_field(kind, attr)
-        ragged, rows_idx = model_rows(m, kind, field, ids)
+        field, ragged, rows_idx = model_rows(m, kind, attr, ids)
         rows_idx = torch.as_tensor(rows_idx, dtype=torch.int64, device=physics.device)
-        t = getattr(physics.env_model, field)
-        rows = t.reshape(t.shape[0], t.shape[1], -1)            # [B, nrows, w] view
-        w = rows.shape[2]
-        shape = (len(rows_idx),) + ((w,) if w > 1 else ())      # bind's per-environment shape
-        if single and not ragged:
-          shape = shape[1:]
+        rows = getattr(physics.env_model, field)                # [B, nrows, *width]
+        k_width = (len(rows_idx),) + rows.shape[2:]
+        shape = k_width[1:] if single and not ragged else k_width     # bind's per-environment shape
         if info.initial_value is None:
           info.initial_value = rows[:, rows_idx].reshape((physics.batch,) + shape).clone()
         current = rows[envs][:, rows_idx].reshape((n,) + shape)
         v = info.variation
         value = v(info.initial_value[envs], current, generator, n) if callable(v) else v
         value = torch.as_tensor(value, dtype=rows.dtype, device=physics.device)
-        rows[envs[:, None], rows_idx[None, :]] = value.expand((n,) + shape).reshape(n, len(rows_idx), w)
+        rows[envs[:, None], rows_idx[None, :]] = value.expand((n,) + shape).reshape((n,) + k_width)
     physics.mark_as_dirty()
 
   def clear(self):
